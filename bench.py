@@ -5,7 +5,7 @@
     python bench.py --impl reference --gpus N --steps K --warmup W
 
 A "step" is one pass of the hot path: C = A + B over this rank's 2^28-element shard
-(weak scaling: every GPU holds 2^28 elements, 3 GiB of operands, far above the 126 MB L2,
+(weak scaling: every GPU holds 2^28 elements, 3 GiB of operands, far above the 50 MB L2,
 so no L2 flush is needed between steps).  One step == one launch of OUR kernel through the
 C ABI (include/b200va.h: b200va_add_f32).
 
@@ -14,19 +14,25 @@ value        whole-job elements/s with operands resident in HBM (CUDA events, ma
 e2e          the same metric through the host-buffer C-ABI call (b200va_stager_add_f32) on
              pinned host arrays: every step copies A and B to the GPU, adds, copies C back;
              e2e.roofline = the same bytes as plain concurrent whole-array copies, measured
-             live on this box at this N (the PCIe / host-DMA ceiling)
+             live on the same machine at this N (the PCIe / host-DMA ceiling)
 e2e_pageable the same call on plain malloc'd arrays -- what the reference's process has --
              first step (page-locks them once) and steady state
-roofline     dominant (only) kernel vs the measured HBM copy peak (MEASURED_PEAKS.json)
+roofline     dominant (only) kernel vs the measured HBM copy peak (MEASURED_PEAKS.json) and vs a
+             pure read stream measured in the same run
 cpu_baseline / --impl reference
              the oracle port (oracle/vadd_oracle.c: the reference ships no source, so kind =
-             "port") timed on this box's host cores, regular AND non-temporal stores, the
+             "port") timed on the host cores, regular AND non-temporal stores, the
              faster reported.  The oracle is never on the product path.
 The other BASELINE.json configs that fit a bench run ride in the same line:
 strong_2p30  configs[2]: global N = 2^30 sharded over the N ranks (2^30/N per GPU), fixed total
 cli_strong_2p30  the same shape through the C++ executable's one-thread-per-GPU path (`vectorAdd --gpus N`),
              run by rank 0 on exactly the GPUs the ranks drove
 loop_2p24    configs[4]: 5000 launches of N = 2^24 in 50-launch CUDA graphs on each GPU
+
+--dump-outputs DIR writes C of the last timed step (rank r > 0: suffix _r<r>) to DIR as float32 .npy:
+the whole vector when it is at most 64 MiB, otherwise the elements at a fixed, seeded sample of
+indices (c_sample.npy, indices in c_sample_index.npy as float64).  Inputs depend only on the
+arguments, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -47,13 +53,15 @@ WORKLOAD = "vectorAdd N=2^28 fp32 per GPU (BASELINE.json configs[1])"     # iden
 INPUTS = "ctr generator (splitmix64 of the global index), seeds 0x0A/0x0B, uniform [0,1)"
 N_PER_GPU = 1 << 28
 CLOCK_PERIOD_MS = 2.0
-STAGE_MODE = 2       # host-path pipeline used for e2e (0 slot streams, 2 lanes: 42.25 vs 42.56 ms, profiles/r01/m_*)
+STAGE_MODE = 2       # host-path pipeline used for e2e (0: one stream per slot, 2: one stream per direction, "lanes")
 BYTES_PER_ELEM = 12  # 4 read A + 4 read B + 4 write C (SURVEY.md section 8(d))
 # oracle.ctr_vadd_digest(1 << 30) / (1 << 24): asserted against the oracle in tests/test_oracle.py
 DIGEST_2P30 = (0x0FD8E36879AED49F, 0x0F23C595)
 DIGEST_2P24 = (0x003F639456AC9687, 0x064A9499)
-READ_ONLY_CEILING_GBPS = 7436.0   # pure read stream (A and B in, nothing out) with the production geometry: profiles/r02/a_channel_skew.jsonl
-LINK_ALONE_MS_PER_2P28 = 40.8   # one GPU's PCIe Gen5 x16 link, 2 GiB in + 1 GiB out concurrently (profiles/r01/l_pcie_probe.jsonl)
+HBM_DATASHEET_GBPS = 3350.0   # H100 SXM data sheet HBM3 bandwidth: a label for the fraction below, never a measurement
+DUMP_MAX_BYTES = 64 << 20
+DUMP_SAMPLE = 1 << 21         # sampled elements when C is larger than DUMP_MAX_BYTES (float32 values + float64 indices)
+DUMP_SEED = 0x5EED
 
 
 # --------------------------------------------------------------------------- clocks
@@ -125,19 +133,24 @@ def measured_peak() -> tuple[float, str]:
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, torch copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md: 6.65 TB/s)"
+        return HBM_DATASHEET_GBPS, "fallback: H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
-def ncu_traffic(kernel: str, n: int) -> tuple[float | None, str | None]:
-    """dram read+write bytes per launch of THE KERNEL THIS RUN LAUNCHED, from the per-kernel table
-    of committed ncu captures (profiles/ncu_summary.json, key "<kernel>@<n>").  None when this
-    kernel/size has no capture -- never another kernel's bytes."""
-    try:
-        table = json.load(open(os.path.join(ROOT, "profiles", "ncu_summary.json")))["kernels"]
-        row = table[f"{kernel}@{n}"]
-        return float(row["dram_bytes_per_launch"]), row.get("source")
-    except Exception:
-        return None, None
+def dump_outputs(out_dir: str, c, rank: int) -> None:
+    """C of the last timed step as float32 .npy: whole if small enough, else a fixed seeded sample."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = f"_r{rank}" if rank else ""
+    n = c.numel()
+    if 4 * n <= DUMP_MAX_BYTES:
+        np.save(os.path.join(out_dir, f"c{sfx}.npy"), c.cpu().numpy().astype(np.float32))
+        return
+    idx = np.unique(np.random.default_rng(DUMP_SEED).integers(0, n, DUMP_SAMPLE, dtype=np.int64))
+    vals = c[torch.from_numpy(idx).to(c.device)].cpu().numpy().astype(np.float32)
+    np.save(os.path.join(out_dir, f"c_sample{sfx}.npy"), vals)
+    np.save(os.path.join(out_dir, f"c_sample_index{sfx}.npy"), idx.astype(np.float64))
 
 
 # --------------------------------------------------------------------------- reference arm
@@ -247,7 +260,7 @@ def time_steps(fn, steps: int, stream, sharding, sampler=None):
 
 
 def pcie_probe(a, b, c, ha, hb, hc, sharding, reps: int = 3) -> float:
-    """The ceiling of the host-buffer step on this box at this rank count: the step's bytes as
+    """The ceiling of the host-buffer step on this machine at this rank count: the step's bytes as
     PLAIN whole-array copies (H2D A, H2D B on one stream, D2H C on another, concurrently), every
     rank at once.  Returns the best-of-reps max-over-ranks milliseconds.  torch copies: none of
     our code is on this path."""
@@ -298,7 +311,7 @@ def cli_strong(gpus: int, cli: str, devices: list[int] | None = None) -> dict:
             return {"error": repr(e)[:200]}
     return {"command": f"vectorAdd --mode resident --gpus {gpus} --n 2^30 --iters 20", "devices": devices, "exit_code": p.returncode,
             "value": r["elements_per_s"], "unit": UNIT, "ms_per_step": r["ms_per_pass"], "mismatches": r["mismatches"],
-            "frac_of_8TBps_nameplate_per_gpu": r["roofline_frac_of_8TBps_per_gpu"],
+            "frac_of_3p35TBps_datasheet_per_gpu": r["roofline_frac_of_3p35TBps_per_gpu"],
             "digest_ok": (int(r["digest_sum"], 16), int(r["digest_xor"], 16)) == DIGEST_2P30}
 
 
@@ -347,6 +360,8 @@ def run_ours(args, emit=print) -> None:
     sampler = ClockSampler(dev_index, args.clock_period_ms * 1e-3)
     ms_total = time_steps(step, args.steps, stream, sharding, sampler)
     launches = int(sharding.sum_over_ranks(args.steps))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, c, rank)
 
     # ---- correctness of what was timed (outside the timed region): bit-exact recompute in
     # HBM plus the order-independent digest, combined over shards
@@ -392,18 +407,17 @@ def run_ours(args, emit=print) -> None:
         # the platform's ceiling for these bytes, live, all ranks at once
         probe_ms = pcie_probe(a, b, c, ha, hb, hc, sharding)
         step_bytes = BYTES_PER_ELEM * n * ws
-        link_ms = LINK_ALONE_MS_PER_2P28 * n / (1 << 28)
         e2e = {"value": ws * n * e2e_steps / (ms_e2e * 1e-3), "unit": UNIT, "h2d_bytes_per_step": 8 * n * ws,
                "d2h_bytes_per_step": 4 * n * ws, "steps": e2e_steps, "ms_per_step": ms_e2e / e2e_steps,
                "path": "b200va_stager_add_f32 " + {0: "copy-engine pipeline, one stream per slot: H2D(A,B) -> add -> D2H(C) per chunk",
                                                    1: "zero-copy kernel over PCIe",
                                                    2: "copy-engine pipeline, one stream per direction (lanes): H2D(A,B) | add | D2H(C)"}[mode],
                "host_memory": "pinned (b200va_host_alloc, GPU-local NUMA node)" + (", write-combined inputs" if args.wc_inputs else ""),
-               "roofline": {"bound": "pcie" if probe_ms <= 1.15 * link_ms else "host-dma",
+               "roofline": {"bound": "pcie / host-dma",
                             "achieved": step_bytes / (ms_e2e / e2e_steps) / 1e6, "peak": step_bytes / probe_ms / 1e6, "unit": "GB/s",
                             "frac": probe_ms / (ms_e2e / e2e_steps), "probe_ms": probe_ms,
                             "peak_source": "live probe in this run: the step's bytes as plain whole-array torch copies, H2D(A,B) and D2H(C) "
-                                           f"concurrently, all {ws} ranks at once, best of 3 (one link alone: {link_ms:.1f} ms, profiles/r01/l_pcie_probe.jsonl)"},
+                                           f"concurrently, all {ws} ranks at once, best of 3"},
                "device_numaGpu_numaA_B_C_per_rank": host_nodes}
         del ha, hb, hc
         for p in (pa, pb, pc):
@@ -472,8 +486,8 @@ def run_ours(args, emit=print) -> None:
                 "us_per_iter": 1e3 * ms_loop_max / iters, "value": ws * m * iters / (ms_loop_max * 1e-3), "unit": UNIT,
                 "algorithmic_GBps_per_gpu": BYTES_PER_ELEM * m * iters / (ms_loop_max * 1e-3) / 1e9,
                 "busy_frac": ms_loop / wall_ms, "wall_ms": wall_ms,
-                "note": "L2-assisted: the 192 MiB footprint is 1.5x the 126 MB L2 and the same buffers are re-read every launch, so part "
-                        "of the traffic is served from L2 -- not an HBM figure (cold-buffer rate: profiles/r02 sweep_n)",
+                "note": "the same buffers are re-read every launch and the 192 MiB footprint is about 4x the 50 MB L2, so a part "
+                        "of the traffic may be served from L2",
                 "kernel": ltune.kernel_name(), "mismatches": lbad,
                 "digest_ok": (va.digest(lc) == DIGEST_2P24) if (first == 0 and m == 1 << 24) else None}
         del la, lb, lc, lp
@@ -508,7 +522,7 @@ def run_ours(args, emit=print) -> None:
         strong = {"config": "BASELINE.json configs[2]: vectorAdd N=2^30 fp32 sharded over the ranks (b200va_shard_range), no collective",
                   "global_n": gn, "n_per_gpu": m, "scaling": "strong", "steps": s_steps, "ms_per_step": s_ms_step,
                   "value": gn * s_steps / (ms_s * 1e-3), "unit": UNIT, "per_gpu_GBps": s_ach, "frac": s_ach / peak,
-                  "frac_of_8TBps_nameplate_per_gpu": s_ach / 8000.0, "kernel": pkg.resolve(variant, m, capi.F_INPUTS_STABLE if args.chain else 0).kernel_name(),
+                  "frac_of_3p35TBps_datasheet_per_gpu": s_ach / HBM_DATASHEET_GBPS, "kernel": pkg.resolve(variant, m, capi.F_INPUTS_STABLE if args.chain else 0).kernel_name(),
                   "mismatches": sbad, "digest_sum": f"{sdig[0]:016x}", "digest_xor": f"{sdig[1]:08x}",
                   "digest_ok": sdig == DIGEST_2P30}
         del sa, sb, sc
@@ -522,7 +536,6 @@ def run_ours(args, emit=print) -> None:
     ms_per_step = ms_total / args.steps
     achieved = BYTES_PER_ELEM * n / (ms_per_step * 1e-3) / 1e9  # per GPU, GB/s
     kname = tune.kernel_name()
-    traffic, traffic_src = ncu_traffic(kname, n)
     grid, block = capi.C.c_uint(), capi.C.c_uint()
     capi.lib.b200va_geometry(capi.C.byref(tune), n, dev_index, capi.C.byref(grid), capi.C.byref(block), None)
     line = {
@@ -533,18 +546,17 @@ def run_ours(args, emit=print) -> None:
                    "sharding": f"weak scaling: global N = {ws} x 2^28, contiguous shards, no collective on the data path",
                    "rank_to_device": "round-robin over NUMA nodes when ranks < GPUs" if not args.identity_mapping else "identity",
                    "device_numa_nodes": dev_nodes, "kernel": tune.as_dict(), "inputs": INPUTS,
-                   "l2": "operands 3 GiB per GPU >> 126 MB L2: inputs larger than L2, no flush between steps",
+                   "l2": "operands 3 GiB per GPU >> 50 MB L2: inputs larger than L2, no flush between steps",
                    "verified": "bit-exact recompute in HBM after the timed region",
                    "digest_sum": f"{dig[0]:016x}", "digest_xor": f"{dig[1]:08x}"},
         "algorithmic_GBps": value * BYTES_PER_ELEM / 1e9,
-        "frac_of_8TBps_nameplate_per_gpu": achieved / 8000.0,
+        "frac_of_3p35TBps_datasheet_per_gpu": achieved / HBM_DATASHEET_GBPS,
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                     "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": BYTES_PER_ELEM * n,
                      "read_only_ceiling_GBps": read_ceiling, "frac_of_read_only_ceiling": achieved / read_ceiling,
                      "read_only_ceiling": "measured in this run: b200va_probe_f32(READ2) -- the production launch geometry loading A and B and storing "
-                                          f"nothing, {probe_steps} launches (committed reference: {READ_ONLY_CEILING_GBPS:.0f} GB/s = 91 % of the 8.18 TB/s pin "
-                                          "rate, profiles/r02/a_channel_skew.jsonl); a harder denominator than the torch copy peak",
+                                          f"nothing, {probe_steps} launches; a harder denominator than the torch copy peak",
                      "kernel": f"b200va::{kname} grid {grid.value} x {block.value} threads (one launch per step)"},
         "clocks": sampler.summary(),
         "gpu_launches": launches,
@@ -608,7 +620,10 @@ def main() -> None:
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip strong_2p30 and loop_2p24")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write C of the last timed step to DIR as .npy (see the module docstring)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
         return

@@ -1,5 +1,5 @@
 /*
- * b200va.h -- C ABI of libb200va.so: the B200 (sm_100a) vectorAdd hot path.
+ * b200va.h -- C ABI of libb200va.so: the H100 (sm_90a) vectorAdd hot path.
  *
  * The reference (ashrafgt/k8s-gpu-hpa) has NO library/plugin API for this path: the
  * kernel is statically linked into the `vectorAdd` executable inside the third-party
@@ -48,7 +48,7 @@ extern "C" {
 #define B200VA_ERR_ALIGN       (-2)   /* pointer not 4-byte aligned                       */
 #define B200VA_ERR_OVERLAP     (-3)   /* C partially overlaps A or B (exact alias is ok)  */
 #define B200VA_ERR_VARIANT     (-4)   /* unknown kernel variant / unsupported tune combo  */
-#define B200VA_ERR_NO_DEVICE   (-5)   /* no CUDA device / not an sm_100 device            */
+#define B200VA_ERR_NO_DEVICE   (-5)   /* no CUDA device / not an sm_90 device             */
 #define B200VA_ERR_VERIFY      (-6)   /* result verification failed (a6)                  */
 #define B200VA_ERR_NOMEM       (-7)   /* host allocation failed                           */
 #define B200VA_ERR_CUDA_BASE   (-1000) /* code = -(1000 + cudaError_t)                    */
@@ -63,8 +63,9 @@ extern "C" {
                                   (n+255)/256 CTAs  (CUDA sample launch geometry, a5)   */
 #define B200VA_K1_VEC128   2   /* 128-bit ld/st.global.v4.f32, unrolled, cache-hinted   */
 #define B200VA_K2_TMA      3   /* cp.async.bulk (TMA) smem ring; tiles handed out by the
-                                  cluster-launch-control scheduler (store_mode 2)        */
-#define B200VA_K3_VEC256   4   /* 256-bit ld/st.global.v8.f32 (PTX 8.8, sm_100)         */
+                                  dynamic tile scheduler (store_mode 2)                  */
+#define B200VA_K3_VEC256   4   /* 32-byte vectors per thread: two adjacent 128-bit
+                                  ld/st.global.v4.f32 (sm_90 has no 256-bit access)     */
 #define B200VA_K4_SCALAR_MLP 5 /* 32-bit accesses, `unroll` (4|8|16) independent loads per array
                                   per thread in flight: the mixed-misalignment path, also
                                   selectable through b200va_add_f32_tuned for A/B runs   */
@@ -80,7 +81,8 @@ typedef struct b200va_tune {
     int stages;       /* TMA: ring depth (2..16)                                        */
     int tile_bytes;   /* TMA: bytes per array per stage (multiple of 2048)              */
     int store_mode;   /* TMA: 0 = st.global from registers, 1 = bulk store from smem,
-                         2 = register stores + cluster-launch-control tile scheduler    */
+                         2 = register stores + dynamic tile scheduler (persistent grid,
+                             tiles claimed from an atomic ticket counter)               */
     int early_loads;  /* vec: what a CTA does about its first tile before the programmatic
                          dependency on the previous launch resolves:
                          1 = issue the loads themselves (only the stores wait).  Requires that
@@ -90,8 +92,9 @@ typedef struct b200va_tune {
                              loads and stores wait.  Always legal (L2 is the coherence point);
                              pays off on data that is not already in L2.                     */
     int scheduler;    /* vec: 0 = hardware block scheduler (one CTA per tile, or the static
-                         persistent split of ctas_per_sm), 1 = cluster launch control:
-                         resident CTAs cancel and take over not-yet-started ones (K1c)   */
+                         persistent split of ctas_per_sm), 1 = dynamic tile scheduler:
+                         a persistent grid whose CTAs claim tiles from an atomic ticket
+                         counter (K1d)                                                  */
 } b200va_tune_t;
 
 typedef struct b200va_devinfo {

@@ -45,18 +45,17 @@ class Tune(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
     def kernel_name(self) -> str:
-        """The kernel this tune launches, as ncu prints it minus the (int)/(bool) casts: the key
-        of the per-kernel table in profiles/ncu_summary.json."""
+        """The kernel this tune launches, as a profiler prints it minus the (int)/(bool) casts."""
         if self.kind == K0_SCALAR:
             return "vadd_scalar"
         if self.kind == K2_TMA:
             hint = int(self.ld_hint == 3)
             if self.store_mode == 2:
-                return f"vadd_tma_clc<{hint},{self.st_hint}>"
+                return f"vadd_tma_dyn<{hint},{self.st_hint}>"
             return f"vadd_tma<{self.store_mode},{hint},{self.st_hint if self.store_mode == 0 else 0}>"
         if self.kind == K4_SCALAR_MLP:
             return f"vadd_scalar_unrolled<{self.unroll}>"
-        name = "vadd_vec_clc" if self.scheduler == 1 else "vadd_vec"
+        name = "vadd_vec_dyn" if self.scheduler == 1 else "vadd_vec"
         return f"{name}<{8 if self.kind == K3_VEC256 else 4},{self.unroll},{self.ld_hint},{self.st_hint},{self.early_loads}>"
 
 

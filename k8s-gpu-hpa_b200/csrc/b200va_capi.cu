@@ -1,6 +1,6 @@
 // b200va_capi.cu -- the C ABI of libb200va.so (declared in include/b200va.h).
 //
-// Host-side dispatch for the sm_100a vectorAdd kernels: argument checking, alignment
+// Host-side dispatch for the sm_90a vectorAdd kernels: argument checking, alignment
 // peeling, geometry resolution, the in-process launch loop, the host-buffer staging
 // pipeline.  Each entry point names the step of the reference's `./vectorAdd` process
 // it replaces (cuda-test-deployment.yaml:18-19; SURVEY.md section 8(a)).
@@ -76,8 +76,8 @@ int dev_info(int device, const b200va_devinfo_t** out)
         dc.info.sm_count = sms;
         dc.info.max_smem_optin = smem;
         dc.info.l2_bytes = l2;
-        // the cubin is sm_100a SASS (+ compute_100a PTX): architecture-specific, it runs on CC 10.0 only
-        dc.rc = (major == 10 && minor == 0) ? B200VA_OK : B200VA_ERR_NO_DEVICE;
+        // the cubin is sm_90a SASS (+ compute_90a PTX): architecture-specific, it runs on CC 9.0 only
+        dc.rc = (major == 9 && minor == 0) ? B200VA_OK : B200VA_ERR_NO_DEVICE;
     });
     if (out) *out = &dc.info;
     return dc.rc;
@@ -90,53 +90,84 @@ int current_dev_info(const b200va_devinfo_t** out)
     return dev_info(device, out);
 }
 
+// Restores the calling thread's current device on every exit path of the entry points that
+// take a `device` argument (include/b200va.h: "restore the caller's current device").
+struct DeviceGuard {
+    int prev = -1;
+    cudaError_t err = cudaSuccess;
+    explicit DeviceGuard(int device)
+    {
+        if (cudaGetDevice(&prev) != cudaSuccess) { prev = -1; cudaGetLastError(); }
+        if (prev != device) err = cudaSetDevice(device);
+    }
+    ~DeviceGuard()
+    {
+        int now = -1;
+        if (prev >= 0 && cudaGetDevice(&now) == cudaSuccess && now != prev) cudaSetDevice(prev);
+    }
+    DeviceGuard(const DeviceGuard&) = delete;
+    DeviceGuard& operator=(const DeviceGuard&) = delete;
+};
+
 // ----------------------------------------------------------------------- vec dispatch
 // libb200va.so carries the production set only (what AUTO and the named variants resolve to,
 // plus close neighbours used by the parity tests); -DB200VA_TUNE_MATRIX (libb200va_tune.so, the
 // A/B tool's library) instantiates every combination of b200va_tune_t.  A combination that is
 // not compiled in makes the pick functions return nullptr -> B200VA_ERR_VARIANT.
 using vec_fn = void (*)(const float*, const float*, float*, size_t, size_t, size_t, size_t);
+using dyn_fn = void (*)(const float*, const float*, float*, size_t, size_t, size_t, size_t, unsigned int*);
+
+// The vec kernel a tune selects: `plain` under the hardware block scheduler, `dyn` under the
+// dynamic tile scheduler (scheduler = 1); at most one is set.
+struct VecFn {
+    vec_fn plain = nullptr;
+    dyn_fn dyn = nullptr;
+    explicit operator bool() const { return plain || dyn; }
+    const void* key() const { return plain ? reinterpret_cast<const void*>(plain) : reinterpret_cast<const void*>(dyn); }
+};
 
 template <int VW, int UNROLL, int LD, int ST>
-vec_fn pick_early_hw(int early)
+VecFn pick_early_hw(int early)
 {
+    VecFn f;
     switch (early) {
-        case 0: return vadd_vec<VW, UNROLL, LD, ST, 0>;
-        case 1: return vadd_vec<VW, UNROLL, LD, ST, 1>;
-        case 2: return vadd_vec<VW, UNROLL, LD, ST, 2>;
+        case 0: f.plain = vadd_vec<VW, UNROLL, LD, ST, 0>; break;
+        case 1: f.plain = vadd_vec<VW, UNROLL, LD, ST, 1>; break;
+        case 2: f.plain = vadd_vec<VW, UNROLL, LD, ST, 2>; break;
     }
-    return nullptr;
+    return f;
 }
 
 template <int VW, int UNROLL, int LD, int ST>
-vec_fn pick_early_clc(int early)
+VecFn pick_early_dyn(int early)
 {
+    VecFn f;
     switch (early) {
-        case 0: return vadd_vec_clc<VW, UNROLL, LD, ST, 0>;
-        case 1: return vadd_vec_clc<VW, UNROLL, LD, ST, 1>;
-        case 2: return vadd_vec_clc<VW, UNROLL, LD, ST, 2>;
+        case 0: f.dyn = vadd_vec_dyn<VW, UNROLL, LD, ST, 0>; break;
+        case 1: f.dyn = vadd_vec_dyn<VW, UNROLL, LD, ST, 1>; break;
+        case 2: f.dyn = vadd_vec_dyn<VW, UNROLL, LD, ST, 2>; break;
     }
-    return nullptr;
+    return f;
 }
 
 template <int VW, int UNROLL, int LD, int ST>
-vec_fn pick_sched(int early, int sched)
+VecFn pick_sched(int early, int sched)
 {
     if (sched == 1) {
 #ifdef B200VA_TUNE_MATRIX
-        return pick_early_clc<VW, UNROLL, LD, ST>(early);
+        return pick_early_dyn<VW, UNROLL, LD, ST>(early);
 #else
         if constexpr (VW == 4 && LD == LD_PLAIN && ST == ST_NA && (UNROLL == 2 || UNROLL == 4))
-            return pick_early_clc<VW, UNROLL, LD, ST>(early);
+            return pick_early_dyn<VW, UNROLL, LD, ST>(early);
         else
-            return nullptr;
+            return VecFn{};
 #endif
     }
     return pick_early_hw<VW, UNROLL, LD, ST>(early);
 }
 
 template <int VW, int UNROLL, int LD>
-vec_fn pick_st(int st, int early, int sched)
+VecFn pick_st(int st, int early, int sched)
 {
     switch (st) {
         case ST_PLAIN: return pick_sched<VW, UNROLL, LD, ST_PLAIN>(early, sched);
@@ -146,11 +177,11 @@ vec_fn pick_st(int st, int early, int sched)
         case ST_NA_EF: return pick_sched<VW, UNROLL, LD, ST_NA_EF>(early, sched);
 #endif
     }
-    return nullptr;
+    return VecFn{};
 }
 
 template <int VW, int UNROLL>
-vec_fn pick_ld(int ld, int st, int early, int sched)
+VecFn pick_ld(int ld, int st, int early, int sched)
 {
     switch (ld) {
         case LD_PLAIN: return pick_st<VW, UNROLL, LD_PLAIN>(st, early, sched);
@@ -162,11 +193,11 @@ vec_fn pick_ld(int ld, int st, int early, int sched)
         case LD_NA_256: return pick_st<VW, UNROLL, LD_NA_256>(st, early, sched);
 #endif
     }
-    return nullptr;
+    return VecFn{};
 }
 
 template <int VW>
-vec_fn pick_unroll(int unroll, int ld, int st, int early, int sched)
+VecFn pick_unroll(int unroll, int ld, int st, int early, int sched)
 {
     switch (unroll) {
         case 1: return pick_ld<VW, 1>(ld, st, early, sched);
@@ -176,16 +207,17 @@ vec_fn pick_unroll(int unroll, int ld, int st, int early, int sched)
         case 8: return pick_ld<VW, 8>(ld, st, early, sched);
 #endif
     }
-    return nullptr;
+    return VecFn{};
 }
 
-vec_fn pick_vec(int vw, int unroll, int ld, int st, int early, int sched)
+VecFn pick_vec(int vw, int unroll, int ld, int st, int early, int sched)
 {
     return vw == 8 ? pick_unroll<8>(unroll, ld, st, early, sched) : pick_unroll<4>(unroll, ld, st, early, sched);
 }
 
 // ----------------------------------------------------------------------- tma dispatch
 using tma_fn = void (*)(const float*, const float*, float*, size_t, size_t, size_t, uint32_t, uint32_t);
+using tma_dyn_fn = void (*)(const float*, const float*, float*, size_t, size_t, size_t, uint32_t, uint32_t, unsigned int*);
 
 #ifdef B200VA_TUNE_MATRIX
 template <int MODE, bool HINT>
@@ -201,30 +233,35 @@ tma_fn pick_tma_st(int st)
 }
 #endif
 
+// store_mode 2: the dynamic tile scheduler, register stores
 template <bool HINT>
-tma_fn pick_tma_clc_st(int st)
+tma_dyn_fn pick_tma_dyn_st(int st)
 {
     switch (st) {
-        case ST_PLAIN: return vadd_tma_clc<HINT, ST_PLAIN>;
-        case ST_NA:    return vadd_tma_clc<HINT, ST_NA>;
+        case ST_PLAIN: return vadd_tma_dyn<HINT, ST_PLAIN>;
+        case ST_NA:    return vadd_tma_dyn<HINT, ST_NA>;
 #ifdef B200VA_TUNE_MATRIX
-        case ST_CS:    return vadd_tma_clc<HINT, ST_CS>;
-        case ST_NA_EF: return vadd_tma_clc<HINT, ST_NA_EF>;
+        case ST_CS:    return vadd_tma_dyn<HINT, ST_CS>;
+        case ST_NA_EF: return vadd_tma_dyn<HINT, ST_NA_EF>;
 #endif
     }
     return nullptr;
 }
 
+tma_dyn_fn pick_tma_dyn(bool l2_hint, int st)
+{
+    return l2_hint ? pick_tma_dyn_st<true>(st) : pick_tma_dyn_st<false>(st);
+}
+
 tma_fn pick_tma(int store_mode, bool l2_hint, int st)
 {
-    if (store_mode == 2)  // cluster-launch-control tile scheduler, register stores
-        return l2_hint ? pick_tma_clc_st<true>(st) : pick_tma_clc_st<false>(st);
 #ifdef B200VA_TUNE_MATRIX
     if (store_mode == 1)  // st hint is meaningless for bulk stores: one instantiation
         return l2_hint ? vadd_tma<1, true, ST_PLAIN> : vadd_tma<1, false, ST_PLAIN>;
     return l2_hint ? pick_tma_st<0, true>(st) : pick_tma_st<0, false>(st);
 #else
-    // the static-split ring (store modes 0/1) lost to the CLC form everywhere: tune library only
+    // the static-split ring (store modes 0/1) is not a production default: the tune library carries its
+    // matrix, this library two forms
     if (store_mode == 1 && !l2_hint) return vadd_tma<1, false, ST_PLAIN>;   // kept: the bulk-store (UBLKCP.G.S) form
     if (store_mode == 0 && !l2_hint && st == ST_NA) return vadd_tma<0, false, ST_NA>;
     return nullptr;
@@ -234,48 +271,45 @@ tma_fn pick_tma(int store_mode, bool l2_hint, int st)
 std::mutex g_attr_mu;
 
 // Opt in to > 48 KiB dynamic shared memory once per (function, device).
-int ensure_smem_optin(tma_fn fn, int device, int bytes)
+int ensure_smem_optin(const void* fn, int device, int bytes)
 {
-    struct Key { tma_fn fn; int device; int bytes; };
+    struct Key { const void* fn; int device; int bytes; };
     static Key seen[256];
     static int n_seen = 0;
     std::lock_guard<std::mutex> lk(g_attr_mu);
     for (int i = 0; i < n_seen; ++i)
         if (seen[i].fn == fn && seen[i].device == device) {
             if (seen[i].bytes >= bytes) return B200VA_OK;
-            CU_TRY(cudaFuncSetAttribute(reinterpret_cast<const void*>(fn),
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+            CU_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
             seen[i].bytes = bytes;
             return B200VA_OK;
         }
-    CU_TRY(cudaFuncSetAttribute(reinterpret_cast<const void*>(fn),
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    CU_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     if (n_seen < 256) seen[n_seen++] = Key{fn, device, bytes};
     return B200VA_OK;
 }
 
 // ----------------------------------------------------------------------- geometry
 // Production choices per size class.  K_AUTO is always the 128-bit kernel; thread count / unroll /
-// cache hints follow the footprint AND what the caller says about the data:
+// cache hints follow the footprint (12 n bytes) AND what the caller says about the data:
 //
-//  default (the same buffers may be launched again: the a1 loop; hot A/B in profiles/r01/{b,c}_ab_2p*.jsonl and
-//  profiles/r02/b_hot_2p*.jsonl -- at these footprints the numbers are L2-assisted, not HBM figures)
-//   n >= 2^25         HBM streaming         512 thr x1, stores skip L1            7.23 TB/s @2^28, 7.14 @2^26, 7.00 @2^25
-//   2^23 < n < 2^25   footprint 1-3 x L2    128 thr x2, L2 evict-first loads      7.34 TB/s @2^24 (7.46 with early loads)
-//   6 Mi <= n <= 2^23 footprint ~ L2        256 thr x2, stores skip L1            11.6 TB/s @2^23 (plain stores: 8.7); early: x4, 14.3
-//   2^21 <= n < 6 Mi  L2-resident           256 thr x2, plain hints (L2 keeps it) 11.7 TB/s @2^22; early: x4, 13.2
-//   n < 2^21          launch-bound          512 thr (>= 2^19) / 128 thr, x1
+//  default (the same buffers may be launched again: the a1 loop)
+//   n >= 2^25         HBM streaming, never L2-resident   512 thr x1, stores skip L1, L2 bulk prefetch ahead of the wait
+//   2^23 < n < 2^25   footprint several x L2             128 thr x2, L2 evict-first loads
+//   6 Mi <= n <= 2^23 footprint ~ 1.5-2 x L2             256 thr x2, stores skip L1
+//   2^21 <= n < 6 Mi  partly L2-resident                 256 thr x2, plain hints (L2 keeps what fits)
+//   n < 2^21          launch-bound                       512 thr (>= 2^19) / 128 thr, x1
 //
-//  B200VA_F_COLD (operands not in L2: the stager's chunks, rotating buffers; profiles/r02/{a,g}_cold_2p*.jsonl, A/B on
-//  >= 4 x L2 of rotating buffer sets).  The launch boundary is what costs here (~1.8 us: the previous grid's tail, then a
-//  full DRAM round trip before the first store), and the always-legal L2 bulk prefetch ahead of griddepcontrol.wait
-//  (early_loads = 2) recovers it without any promise from the caller:
-//   n >= 12 Mi         512 thr x1   7.08 TB/s @2^24          (r01 hot-tuned class: 6.46; plain 512 x1: 6.81)
-//   3 Mi <= n < 12 Mi  512 thr x2   6.95 @2^22, 7.06 @2^23   (5.75 / 6.26; plain 256/512 x1: 5.83 / 6.45)
-//   n < 3 Mi           256 thr x1   4.49 @2^20, 5.87 @2^21   (3.50 / 4.62)
-//  B200VA_F_COLD | B200VA_F_INPUTS_STABLE: from 3 Mi the prefetch form is already the best; below, register loads
-//  ahead of the wait (early_loads = 1) are: 256 thr x4 6.91 TB/s @2^21, 128 thr x2 6.67 @2^20.
-//  n >= 2^25 is never L2-resident, so it always takes the prefetch form (7.25 vs 7.20 TB/s @2^27, 7.22 vs 7.20 @2^28).
+//  B200VA_F_COLD (operands not in L2: the stager's chunks, rotating buffers).  The launch boundary is what
+//  costs here (the previous grid's tail, then a full DRAM round trip before the first store), and the
+//  always-legal L2 bulk prefetch ahead of griddepcontrol.wait (early_loads = 2) hides it without any promise
+//  from the caller:
+//   n >= 12 Mi         512 thr x1
+//   3 Mi <= n < 12 Mi  512 thr x2
+//   n < 3 Mi           256 thr x1
+//  B200VA_F_COLD | B200VA_F_INPUTS_STABLE: from 3 Mi the prefetch form; below, register loads ahead of the
+//  wait (early_loads = 1): 256 thr x4 from 1.5 Mi, 128 thr x2 from 0.5 Mi.
+//  The class boundaries below 2^25 were chosen against the footprint; the 2^28 class is the one bench.py times.
 void default_tune(int variant, size_t n, b200va_tune_t* t, unsigned flags = 0)
 {
     std::memset(t, 0, sizeof *t);
@@ -287,7 +321,7 @@ void default_tune(int variant, size_t n, b200va_tune_t* t, unsigned flags = 0)
             t->threads = 256;
             t->unroll = 1;
             return;
-        case B200VA_K2_TMA:               // TMA ring + cluster-launch-control scheduler (profiles/r01/i_ab_*)
+        case B200VA_K2_TMA:               // TMA ring + dynamic tile scheduler
             t->kind = B200VA_K2_TMA;
             t->threads = n >= (size_t{1} << 25) ? 512 : 128;   // consumer threads (+32 producer)
             t->ctas_per_sm = 1;
@@ -368,7 +402,9 @@ struct Geometry {
     size_t smem = 0, ntiles = 0;
 };
 
-int plan_geometry(const b200va_tune_t& t, const b200va_devinfo_t* di, size_t n, size_t nvec, Geometry* g)
+// `resident`: CTAs of the selected kernel that fit on one SM at once (the occupancy calculator's
+// answer); it sizes the persistent grid of the dynamic tile scheduler.
+int plan_geometry(const b200va_tune_t& t, const b200va_devinfo_t* di, size_t n, size_t nvec, int resident, Geometry* g)
 {
     if (t.kind == B200VA_K0_SCALAR) {
         const size_t blocks = (n + 255) / 256;
@@ -383,14 +419,17 @@ int plan_geometry(const b200va_tune_t& t, const b200va_devinfo_t* di, size_t n, 
         if (t.tile_bytes < 2048 || (t.tile_bytes & 2047)) return B200VA_ERR_VARIANT;
         if (t.st_hint < 0 || t.st_hint >= ST_HINTS) return B200VA_ERR_VARIANT;
         if (t.store_mode < 0 || t.store_mode > 2) return B200VA_ERR_VARIANT;
-        // ring + full/empty barriers; the CLC form adds a barrier, a 16-B response and a tile slot per stage
+        // ring + full/empty barriers; the dynamic-scheduler form adds a tile slot per stage
         const long long smem = static_cast<long long>(t.stages) * 2 * t.tile_bytes +
-                               (t.store_mode == 2 ? 44LL * t.stages + 16 : 16LL * t.stages);
+                               (t.store_mode == 2 ? 20LL : 16LL) * t.stages;
         if (smem > di->max_smem_optin) return B200VA_ERR_VARIANT;
         g->smem = static_cast<size_t>(smem);
         g->ntiles = (nvec * 16u + t.tile_bytes - 1) / t.tile_bytes;
         size_t grid = static_cast<size_t>(di->sm_count) * (t.ctas_per_sm > 0 ? t.ctas_per_sm : 1);
-        if (t.store_mode == 2) grid = g->ntiles;          // one CTA per tile; resident CTAs cancel the rest
+        if (t.store_mode == 2) {                          // persistent: every CTA that fits at once, tiles by ticket
+            if (g->ntiles > 0x7fffffffull) return B200VA_ERR_INVALID;
+            grid = static_cast<size_t>(di->sm_count) * static_cast<size_t>(resident > 0 ? resident : 1);
+        }
         if (grid > 0x7fffffffull) return B200VA_ERR_INVALID;
         if (grid > g->ntiles) grid = g->ntiles;
         g->grid = static_cast<unsigned>(grid ? grid : 1);
@@ -405,7 +444,11 @@ int plan_geometry(const b200va_tune_t& t, const b200va_devinfo_t* di, size_t n, 
     const size_t tile_vecs = static_cast<size_t>(t.threads) * t.unroll;
     g->ntiles = (nvec + tile_vecs - 1) / tile_vecs;
     size_t grid = g->ntiles;
-    if (t.scheduler == 1 && grid > 0x7fffffffull) return B200VA_ERR_INVALID;   // CLC: one CTA per tile, 32-bit tile index
+    if (t.scheduler == 1) {                               // persistent grid, 32-bit tile index
+        if (grid > 0x7fffffffull) return B200VA_ERR_INVALID;
+        const size_t cap = static_cast<size_t>(di->sm_count) * static_cast<size_t>(resident > 0 ? resident : 1);
+        if (grid > cap) grid = cap;
+    }
     if (t.ctas_per_sm > 0) {
         const size_t cap = static_cast<size_t>(di->sm_count) * t.ctas_per_sm;
         if (grid > cap) grid = cap;
@@ -413,6 +456,52 @@ int plan_geometry(const b200va_tune_t& t, const b200va_devinfo_t* di, size_t n, 
     if (grid > 0x7fffffffull) grid = 0x7fffffffull;   // the kernel loops tile += gridDim.x
     g->grid = static_cast<unsigned>(grid ? grid : 1);
     g->block = static_cast<unsigned>(t.threads);
+    return B200VA_OK;
+}
+
+// Ticket counters of the dynamic tile scheduler: a ring of kSchedSlots two-word slots per device,
+// zeroed once and handed out round-robin, one per launch; the kernel's last CTA zeroes its slot
+// again (b200va_ptx.cuh: sched_retire).  Launches on one stream are ordered (every counter access
+// follows griddepcontrol.wait), so a slot is only ever shared by launches that are kSchedSlots
+// apart in issue order and run concurrently on different streams.
+constexpr unsigned kSchedSlots = 4096;
+
+struct SchedPool {
+    std::once_flag once;
+    int rc = B200VA_OK;
+    unsigned int* ctr = nullptr;
+    std::atomic<unsigned> next{0};
+};
+SchedPool g_sched[kMaxDevices];
+
+int sched_slot(int device, unsigned int** out)
+{
+    SchedPool& p = g_sched[device];
+    std::call_once(p.once, [&] {
+        void* d = nullptr;
+        cudaError_t e = cudaMalloc(&d, size_t{kSchedSlots} * 2 * sizeof(unsigned int));
+        if (e == cudaSuccess) e = cudaMemset(d, 0, size_t{kSchedSlots} * 2 * sizeof(unsigned int));
+        if (e != cudaSuccess) { cudaGetLastError(); if (d) cudaFree(d); p.rc = cuda_err(e); return; }
+        p.ctr = static_cast<unsigned int*>(d);
+    });
+    if (p.rc != B200VA_OK) return p.rc;
+    if (out) *out = p.ctr + 2 * (p.next.fetch_add(1, std::memory_order_relaxed) % kSchedSlots);
+    return B200VA_OK;
+}
+
+// CTAs of `fn` (block threads, smem dynamic bytes) that are resident on one SM at once.
+int resident_ctas(const void* fn, unsigned block, size_t smem, int* out)
+{
+    thread_local const void* last_fn = nullptr;
+    thread_local unsigned last_block = 0;
+    thread_local size_t last_smem = 0;
+    thread_local int last = 0;
+    if (fn != last_fn || block != last_block || smem != last_smem) {
+        int k = 0;
+        CU_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k, fn, static_cast<int>(block), smem));
+        last_fn = fn; last_block = block; last_smem = smem; last = k;
+    }
+    *out = last > 0 ? last : 1;
     return B200VA_OK;
 }
 
@@ -512,29 +601,49 @@ int launch(const float* dA, const float* dB, float* dC, size_t n, b200va_tune_t 
     if (vw == 0) {  // the scalar control
         b200va_tune_t k0{};
         k0.kind = B200VA_K0_SCALAR;
-        RC_TRY(plan_geometry(k0, di, n, 0, &g));
+        RC_TRY(plan_geometry(k0, di, n, 0, 1, &g));
         // the control keeps the sample's plain launch (no programmatic dependent launch)
         vadd_scalar<<<g.grid, g.block, 0, stream>>>(dA, dB, dC, n);
         return cuda_err(cudaGetLastError());
     }
     if (head > n) head = n;
     const size_t nvec = (n - head) / static_cast<size_t>(vw);
-    RC_TRY(plan_geometry(t, di, n, nvec, &g));
 
     if (t.kind == B200VA_K2_TMA) {
+        if (t.store_mode == 2) {
+            tma_dyn_fn fn = pick_tma_dyn(t.ld_hint == LD_NA_EF, t.st_hint);
+            if (!fn) return B200VA_ERR_VARIANT;
+            RC_TRY(plan_geometry(t, di, n, nvec, 1, &g));     // validates the tune and sizes the ring
+            RC_TRY(ensure_smem_optin(reinterpret_cast<const void*>(fn), di->device, static_cast<int>(g.smem)));
+            int resident = 1;
+            RC_TRY(resident_ctas(reinterpret_cast<const void*>(fn), g.block, g.smem, &resident));
+            RC_TRY(plan_geometry(t, di, n, nvec, resident, &g));
+            unsigned int* ctr = nullptr;
+            RC_TRY(sched_slot(di->device, &ctr));
+            return launch_kernel(fn, g.grid, g.block, g.smem, stream, dA, dB, dC, n, head, nvec,
+                                 static_cast<uint32_t>(t.tile_bytes), static_cast<uint32_t>(t.stages), ctr);
+        }
+        RC_TRY(plan_geometry(t, di, n, nvec, 1, &g));
         tma_fn fn = pick_tma(t.store_mode, t.ld_hint == LD_NA_EF, t.st_hint);
         if (!fn) return B200VA_ERR_VARIANT;
-        RC_TRY(ensure_smem_optin(fn, di->device, static_cast<int>(g.smem)));
+        RC_TRY(ensure_smem_optin(reinterpret_cast<const void*>(fn), di->device, static_cast<int>(g.smem)));
         return launch_kernel(fn, g.grid, g.block, g.smem, stream, dA, dB, dC, n, head, nvec,
                              static_cast<uint32_t>(t.tile_bytes), static_cast<uint32_t>(t.stages));
     }
     // early register loads (1) read A and B while the previous launch may still be running: never when C aliases
     // an input -- the always-legal L2 prefetch (2) takes their place
     const int early = (t.early_loads == 1 && aliased) ? 2 : t.early_loads;
-    vec_fn fn = pick_vec(vw, t.unroll, t.ld_hint, t.st_hint, early, t.scheduler);
+    RC_TRY(plan_geometry(t, di, n, nvec, 1, &g));             // validates the tune before a kernel is picked
+    const VecFn fn = pick_vec(vw, t.unroll, t.ld_hint, t.st_hint, early, t.scheduler);
     if (!fn) return B200VA_ERR_VARIANT;
-    if (g.block > 256) RC_TRY(check_block_size(fn, g.block));   // deep unrolls: the CTA size is register-limited
-    return launch_kernel(fn, g.grid, g.block, 0, stream, dA, dB, dC, n, head, nvec, g.ntiles);
+    if (g.block > 256) RC_TRY(check_block_size(fn.key(), g.block));   // deep unrolls: the CTA size is register-limited
+    if (fn.plain) return launch_kernel(fn.plain, g.grid, g.block, 0, stream, dA, dB, dC, n, head, nvec, g.ntiles);
+    int resident = 1;
+    RC_TRY(resident_ctas(fn.key(), g.block, 0, &resident));
+    RC_TRY(plan_geometry(t, di, n, nvec, resident, &g));
+    unsigned int* ctr = nullptr;
+    RC_TRY(sched_slot(di->device, &ctr));
+    return launch_kernel(fn.dyn, g.grid, g.block, 0, stream, dA, dB, dC, n, head, nvec, g.ntiles, ctr);
 }
 
 unsigned support_grid(const b200va_devinfo_t* di, size_t n, int threads)
@@ -577,7 +686,7 @@ int launch_stream_typed(const void* dA, const void* dB, void* dC, size_t n, doub
     bool skip_l1_stores = false;
     if (m >= (size_t{1} << 25)) {
         // three-array ops like the add: 512 x 1; two-array ops (copy, scale) want twice the bytes in
-        // flight per thread: 1024 x 2 is 7.04 TB/s vs 6.41 (profiles/r01/r_stream_geometry.jsonl)
+        // flight per thread: 1024 x 2
         threads = binary ? 512 : 1024;
         unroll = binary ? 1 : 2;
         skip_l1_stores = true;
@@ -585,7 +694,7 @@ int launch_stream_typed(const void* dA, const void* dB, void* dC, size_t n, doub
     else if (m >= (size_t{1} << 21)) { threads = 256; unroll = 2; }
     else if (m >= (size_t{1} << 19)) { threads = 512; }
 #ifdef B200VA_TUNE_MATRIX
-    // development knob for profiles/ (tune library only): B200VA_STREAM_GEOMETRY="threads,unroll,skip_l1_stores"
+    // development knob for A/B runs (tune library only): B200VA_STREAM_GEOMETRY="threads,unroll,skip_l1_stores"
     static const struct Override { int threads = 0, unroll = 0, na = 0; } ov = [] {
         Override o;
         if (const char* e = std::getenv("B200VA_STREAM_GEOMETRY")) std::sscanf(e, "%d,%d,%d", &o.threads, &o.unroll, &o.na);
@@ -642,7 +751,7 @@ const char* b200va_strerror(int code)
         case B200VA_ERR_ALIGN:     return "pointer not 4-byte aligned";
         case B200VA_ERR_OVERLAP:   return "output partially overlaps an input";
         case B200VA_ERR_VARIANT:   return "unknown kernel variant or unsupported geometry";
-        case B200VA_ERR_NO_DEVICE: return "no sm_100 CUDA device";
+        case B200VA_ERR_NO_DEVICE: return "no sm_90 CUDA device";
         case B200VA_ERR_VERIFY:    return "result verification failed";
         case B200VA_ERR_NOMEM:     return "host allocation failed";
     }
@@ -688,7 +797,20 @@ int b200va_geometry(const b200va_tune_t* tune, size_t n, int device, unsigned* g
     RC_TRY(dev_info(device, &di));
     Geometry g;
     const size_t vw = tune->kind == B200VA_K3_VEC256 ? 8 : 4;
-    RC_TRY(plan_geometry(*tune, di, n, n / vw, &g));
+    RC_TRY(plan_geometry(*tune, di, n, n / vw, 1, &g));
+    const void* dyn = nullptr;                    // the dynamic scheduler's grid depends on the kernel's occupancy
+    if (tune->kind == B200VA_K2_TMA && tune->store_mode == 2)
+        dyn = reinterpret_cast<const void*>(pick_tma_dyn(tune->ld_hint == LD_NA_EF, tune->st_hint));
+    else if ((tune->kind == B200VA_K1_VEC128 || tune->kind == B200VA_K3_VEC256) && tune->scheduler == 1)
+        dyn = pick_vec(static_cast<int>(vw), tune->unroll, tune->ld_hint, tune->st_hint, tune->early_loads, 1).key();
+    if (dyn) {
+        DeviceGuard guard(device);
+        CU_TRY(guard.err);
+        if (g.smem) RC_TRY(ensure_smem_optin(dyn, device, static_cast<int>(g.smem)));
+        int resident = 1;
+        RC_TRY(resident_ctas(dyn, g.block, g.smem, &resident));
+        RC_TRY(plan_geometry(*tune, di, n, n / vw, resident, &g));
+    }
     *grid = g.grid;
     *block = g.block;
     if (dyn_smem_bytes) *dyn_smem_bytes = static_cast<unsigned>(g.smem);
@@ -792,6 +914,10 @@ int b200va_loop_create(b200va_loop_t** out, const float* dA, const float* dB, fl
     default_tune(variant, n, &l->tune);
     cudaError_t e = cudaGetDevice(&l->device);
     if (e != cudaSuccess) { delete l; return cuda_err(e); }
+    if (l->tune.scheduler == 1 || (l->tune.kind == B200VA_K2_TMA && l->tune.store_mode == 2)) {
+        const int rc = sched_slot(l->device, nullptr);    // allocate the ticket counters before any capture
+        if (rc != B200VA_OK) { delete l; return rc; }
+    }
     if (l->batch > 1 && n > 0) {
         cudaStream_t cap = nullptr;
         e = cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking);
@@ -1004,25 +1130,6 @@ int b200va_shard_range(size_t n, int world, int rank, size_t* begin, size_t* end
 }
 
 // ------------------------------------------------------------------ host-buffer path
-// Restores the calling thread's current device on every exit path of the entry points that
-// take a `device` argument (include/b200va.h: "restore the caller's current device").
-struct DeviceGuard {
-    int prev = -1;
-    cudaError_t err = cudaSuccess;
-    explicit DeviceGuard(int device)
-    {
-        if (cudaGetDevice(&prev) != cudaSuccess) { prev = -1; cudaGetLastError(); }
-        if (prev != device) err = cudaSetDevice(device);
-    }
-    ~DeviceGuard()
-    {
-        int now = -1;
-        if (prev >= 0 && cudaGetDevice(&now) == cudaSuccess && now != prev) cudaSetDevice(prev);
-    }
-    DeviceGuard(const DeviceGuard&) = delete;
-    DeviceGuard& operator=(const DeviceGuard&) = delete;
-};
-
 // Fork-join pool for the pageable path: T persistent workers, each copies one slice.
 // Construction may throw (std::system_error from std::thread under a pids limit, bad_alloc):
 // make_copy_pool() catches and degrades, nothing propagates through the C ABI.
@@ -1303,7 +1410,7 @@ int b200va_stager_create(b200va_stager_t** out, int device, size_t chunk_elems, 
 {
     if (!out) return B200VA_ERR_INVALID;
     *out = nullptr;
-    if (chunk_elems == 0) chunk_elems = size_t{1} << 25;   // 128 MiB per array per slot (tapered tail: profiles/r01/u_*, v_*)
+    if (chunk_elems == 0) chunk_elems = size_t{1} << 25;   // 128 MiB per array per slot (the lanes pipeline tapers the tail)
     if (depth == 0) depth = 3;
     if (depth < 1 || depth > 16) return B200VA_ERR_INVALID;
     chunk_elems = (chunk_elems + 63) & ~size_t{63};        // slots stay 256-B aligned

@@ -1,4 +1,4 @@
-// b200va_kernels.cuh -- the sm_100a kernels of the vectorAdd hot path.
+// b200va_kernels.cuh -- the sm_90a kernels of the vectorAdd hot path.
 //
 // What they replace: the image's `vectorAdd` kernel (C[i] = A[i] + B[i], one element
 // per thread, 256-thread CTAs), which the reference only invokes
@@ -12,11 +12,12 @@
 //   K1  vadd_vec<4,...>  128-bit LDG/STG, UNROLL independent vectors per thread per
 //                        array in flight, cache-hinted, tile-strided (optionally
 //                        persistent).
-//   K3  vadd_vec<8,...>  same with 256-bit LDG.E.256/STG.E.256 (PTX 8.8, sm_100).
-//   K1c vadd_vec_clc     the K1/K3 tile body with Blackwell's cluster-launch-control
-//                        scheduler: resident CTAs cancel not-yet-started CTAs of the grid
-//                        and take over their tiles (no CTA relaunch per tile).
-//   EARLY (K1/K3/K1c)    what a CTA does about its first tile BEFORE the programmatic dependency
+//   K3  vadd_vec<8,...>  same with 32-byte vectors per thread (two adjacent LDG.E.128 /
+//                        STG.E.128: sm_90 has no 256-bit global access).
+//   K1d vadd_vec_dyn     the K1/K3 tile body on a persistent grid with a dynamic tile
+//                        scheduler: CTAs take the next unclaimed tile from an atomic ticket
+//                        counter (no CTA relaunch per tile).
+//   EARLY (K1/K3/K1d)    what a CTA does about its first tile BEFORE the programmatic dependency
 //                        on the previous launch resolves (griddepcontrol.wait):
 //                        1  issues the loads themselves; only the stores wait.  Legal when the
 //                           previous launch on the stream does not write A or B (the launch
@@ -30,16 +31,15 @@
 //                        copies of an A tile and a B tile into a `stages`-deep smem ring
 //                        (mbarrier complete_tx); consumer warps add from smem and either
 //                        store from registers or write back in place and bulk-store.
-//   K2c vadd_tma_clc     the same ring with Blackwell's cluster-launch-control scheduler:
-//                        one CTA per tile in the grid, resident CTAs cancel and take over
-//                        the not-yet-started ones (dynamic balance, persistent ring).
+//   K2d vadd_tma_dyn     the same ring with the dynamic tile scheduler (dynamic balance,
+//                        persistent ring).
 //
 // Ragged sizes / alignment: pointers need only 4-byte alignment.  `head` scalar
 // elements are peeled so the vector body is 16/32-byte aligned, the < VW tail is
 // scalar; both are done by CTA 0 of the same launch (one launch per call, always).
 // If A, B and C share no 16-byte phase there is no vector body: vadd_scalar_unrolled
-// keeps 16 independent 4-byte loads per thread in flight instead (7.19 TB/s at 2^28 --
-// bytes in flight, not access width, is what saturates the HBM).
+// keeps 16 independent 4-byte loads per thread in flight instead (bytes in flight, not
+// access width, is what saturates the HBM).
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -193,29 +193,20 @@ __global__ void vadd_vec(const float* A, const float* B, float* C, size_t n, siz
     if (blockIdx.x == 0) add_edges(A, B, C, n, head, head + nvec * VW, threadIdx.x);
 }
 
-// ------------------------------------------------------------------------------ K1c
-// The vec tile body under the cluster-launch-control scheduler.  Grid = one CTA per tile;
-// a running CTA, before it touches its tile, asks the hardware to cancel one CTA that has
-// not started yet (try_cancel, answered through the async proxy into shared memory and
-// counted on an mbarrier) and -- after its own tile -- processes the cancelled CTA's tile
-// instead of exiting.  The request's latency hides behind the tile's loads.  One response
-// slot: every thread reads it, the CTA barrier orders those reads before thread 0 re-arms it.
+// ------------------------------------------------------------------------------ K1d
+// The vec tile body under the dynamic tile scheduler (b200va_ptx.cuh: sched_next_tile).  The
+// grid is persistent (as many CTAs as are resident at once); a CTA starts on tile blockIdx.x and
+// then takes the next unclaimed tile from the launch's ticket counter instead of exiting, so
+// CTAs that see shorter memory latency simply do more tiles.  Thread 0 asks for the next tile
+// before the current one's loads when the dependency wait is behind it, and publishes the
+// answer through shared memory; the CTA barrier orders every read of the slot before the next write.
 template <int VW, int UNROLL, int LD, int ST, int EARLY>
-__global__ void vadd_vec_clc(const float* A, const float* B, float* C, size_t n, size_t head,
-                             size_t nvec, size_t ntiles)
+__global__ void vadd_vec_dyn(const float* A, const float* B, float* C, size_t n, size_t head,
+                             size_t nvec, size_t ntiles, unsigned int* sched)
 {
-    __shared__ __align__(16) unsigned char resp[16];
-    __shared__ __align__(8) unsigned long long bar_storage;
-    const uint32_t resp_s = smem_u32(resp), bar = smem_u32(&bar_storage);
+    __shared__ uint32_t next_s;
     uint64_t pol = 0;
     if constexpr (LD == LD_NA_EF || ST == ST_NA_EF) pol = l2_evict_first_policy();
-
-    if (threadIdx.x == 0) {
-        mbar_init(bar, 1u);
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    __syncthreads();
 
     const float* a = A + head;
     const float* b = B + head;
@@ -226,27 +217,24 @@ __global__ void vadd_vec_clc(const float* A, const float* B, float* C, size_t n,
     bool waited = EARLY != 1;
     if constexpr (EARLY != 1) pdl_wait();
 
-    uint32_t tile = blockIdx.x, ph = 0;
+    uint32_t tile = blockIdx.x;
     while (true) {
-        if (threadIdx.x == 0) {                           // ask for the tile after this one
-            fence_proxy_async_smem();
-            mbar_arrive_expect_tx(bar, 16u);
-            clc_try_cancel(resp_s, bar);
-        }
+        const bool ask_early = waited;                    // the counter is touched only after the wait
+        if (threadIdx.x == 0 && ask_early) next_s = sched_next_tile(sched);
         if (tile < ntiles) vec_tile<VW, UNROLL, LD, ST>(a, b, c, tile, tile_vecs, nvec, pol, waited);
-        if (tile == 0) {                                  // edges travel with tile 0, whoever runs it
+        if (tile == 0) {                                  // edges travel with tile 0
             if (!waited) { pdl_wait(); waited = true; }
             add_edges(A, B, C, n, head, head + nvec * VW, threadIdx.x);
         }
-        mbar_wait(bar, ph);
-        ph ^= 1u;
-        uint32_t next = 0;
-        const bool ok = clc_query(resp_s, next);
-        __syncthreads();                                  // all reads of the slot precede its re-arm
-        if (!ok) break;
+        if (!waited) { pdl_wait(); waited = true; }
+        if (threadIdx.x == 0 && !ask_early) next_s = sched_next_tile(sched);
+        __syncthreads();
+        const uint32_t next = next_s;
+        __syncthreads();                                  // all reads of the slot precede its next write
+        if (next >= ntiles) break;
         tile = next;
     }
-    if (!waited) pdl_wait();
+    if (threadIdx.x == 0) sched_retire(sched);
 }
 
 // ------------------------------------------------------------------------------ K2
@@ -373,34 +361,28 @@ vadd_tma(const float* A, const float* B, float* C, size_t n, size_t head, size_t
     }
 }
 
-// ------------------------------------------------------------------------------ K2c
-// The TMA ring with Blackwell's cluster-launch-control tile scheduler.  The grid has one
-// CTA per tile, but only as many CTAs as fit are ever resident: each resident CTA's
-// producer lane, besides streaming its own tile through the ring, keeps `stages`
-// try_cancel requests in flight; every success hands it the index of a CTA that has not
-// started yet, whose tile it then loads into the next free stage.  Work is therefore
-// balanced dynamically across SMs (a static persistent split costs ~10 % here because the
-// SMs do not all see the same memory latency) while the ring, the barriers and the CTA
-// stay alive.  Consumers learn each stage's tile index from shared memory; a sentinel
-// ends them.  Register stores only (STORE_MODE 0 of vadd_tma).
+// ------------------------------------------------------------------------------ K2d
+// The TMA ring with the dynamic tile scheduler.  The grid is persistent (as many CTAs as fit
+// at once); each CTA's producer lane streams tile blockIdx.x and then whatever tile the launch's
+// ticket counter hands it next into the next free stage.  Work is therefore balanced dynamically
+// across SMs (a static persistent split leaves the SMs that see longer memory latency as the
+// tail) while the ring, the barriers and the CTA stay alive.  Consumers learn each stage's tile
+// index from shared memory; a sentinel ends them.  Register stores only (STORE_MODE 0 of vadd_tma).
 template <bool L2_HINT, int ST>
 __global__ void __launch_bounds__(1024, 1)
-vadd_tma_clc(const float* A, const float* B, float* C, size_t n, size_t head, size_t nvec4,
-             uint32_t tile_bytes, uint32_t stages)
+vadd_tma_dyn(const float* A, const float* B, float* C, size_t n, size_t head, size_t nvec4,
+             uint32_t tile_bytes, uint32_t stages, unsigned int* sched)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     const uint32_t smem_base = smem_u32(smem);
-    const uint32_t bar_base = smem_base + stages * 2u * tile_bytes;       // full[], empty[], clc_bar[]
-    const uint32_t clc_base = (bar_base + 3u * stages * 8u + 15u) & ~15u; // 16-byte aligned responses
-    const uint32_t slot_base = clc_base + stages * 16u;                   // uint32 tile index per stage
+    const uint32_t bar_base = smem_base + stages * 2u * tile_bytes;       // full[], empty[]
+    const uint32_t slot_base = bar_base + 2u * stages * 8u;               // uint32 tile index per stage
     const uint32_t n_cons = blockDim.x - 32u;
     const uint32_t n_cons_warps = n_cons >> 5;
     constexpr uint32_t kDone = 0xffffffffu;
 
     auto full_bar = [&](uint32_t s) { return bar_base + s * 8u; };
     auto empty_bar = [&](uint32_t s) { return bar_base + (stages + s) * 8u; };
-    auto clc_bar = [&](uint32_t s) { return bar_base + (2u * stages + s) * 8u; };
-    auto clc_resp = [&](uint32_t s) { return clc_base + s * 16u; };
     auto tile_a = [&](uint32_t s) { return smem_base + s * 2u * tile_bytes; };
     auto tile_b = [&](uint32_t s) { return smem_base + s * 2u * tile_bytes + tile_bytes; };
     volatile uint32_t* tile_slot = reinterpret_cast<volatile uint32_t*>(smem + (slot_base - smem_base));
@@ -409,7 +391,6 @@ vadd_tma_clc(const float* A, const float* B, float* C, size_t n, size_t head, si
         for (uint32_t s = 0; s < stages; ++s) {
             mbar_init(full_bar(s), 1u);
             mbar_init(empty_bar(s), n_cons_warps);
-            mbar_init(clc_bar(s), 1u);
         }
         mbar_fence_init();
         fence_proxy_async_smem();
@@ -420,6 +401,7 @@ vadd_tma_clc(const float* A, const float* B, float* C, size_t n, size_t head, si
     const unsigned char* b = reinterpret_cast<const unsigned char*>(B + head);
     unsigned char* c = reinterpret_cast<unsigned char*>(C + head);
     const size_t body_bytes = nvec4 * 16u;
+    const size_t ntiles = (body_bytes + tile_bytes - 1) / tile_bytes;
 
     uint64_t pol = 0;
     if constexpr (L2_HINT || ST == ST_NA_EF) pol = l2_evict_first_policy();
@@ -429,57 +411,22 @@ vadd_tma_clc(const float* A, const float* B, float* C, size_t n, size_t head, si
     if (threadIdx.x < 32) {
         if (threadIdx.x == 0) {
             // ---------------------------------------------------- producer + scheduler
-            for (uint32_t j = 0; j < stages; ++j) {               // `stages` requests in flight
-                mbar_arrive_expect_tx(clc_bar(j), 16u);
-                clc_try_cancel(clc_resp(j), clc_bar(j));
-            }
-            uint32_t outstanding = stages, consumed = 0;
-            bool failed = false;
-            uint32_t tile = blockIdx.x, s = 0, ph = 0;
-            while (body_bytes != 0) {                             // (n < 4: only the scalar edges exist)
+            uint32_t s = 0, ph = 0;
+            for (size_t tile = blockIdx.x; tile < ntiles; tile = sched_next_tile(sched)) {
                 mbar_wait(empty_bar(s), ph ^ 1u);
-                const size_t off = static_cast<size_t>(tile) * tile_bytes;
+                const size_t off = tile * tile_bytes;
                 const size_t left = body_bytes - off;
                 const uint32_t bytes = left < tile_bytes ? static_cast<uint32_t>(left) : tile_bytes;
-                tile_slot[s] = tile;                              // published by the arrive below (release)
+                tile_slot[s] = static_cast<uint32_t>(tile);       // published by the arrive below (release)
                 mbar_arrive_expect_tx(full_bar(s), 2u * bytes);
                 bulk_g2s<L2_HINT>(tile_a(s), a + off, bytes, full_bar(s), pol);
                 bulk_g2s<L2_HINT>(tile_b(s), b + off, bytes, full_bar(s), pol);
                 if (++s == stages) { s = 0; ph ^= 1u; }
-
-                // next tile: the oldest outstanding response; after the first failure nothing
-                // is re-armed, but every outstanding response is still drained before exit
-                bool have_next = false;
-                while (outstanding > 0 && !have_next) {
-                    const uint32_t j = consumed % stages;
-                    mbar_wait(clc_bar(j), (consumed / stages) & 1u);
-                    uint32_t next = 0;
-                    const bool ok = clc_query(clc_resp(j), next);
-                    ++consumed;
-                    --outstanding;
-                    if (ok) {
-                        tile = next;
-                        have_next = true;
-                        if (!failed) {
-                            fence_proxy_async_smem();             // the generic-proxy read of the slot precedes its async re-write
-                            mbar_arrive_expect_tx(clc_bar(j), 16u);
-                            clc_try_cancel(clc_resp(j), clc_bar(j));
-                            ++outstanding;
-                        }
-                    } else {
-                        failed = true;
-                    }
-                }
-                if (!have_next) break;
-            }
-            while (outstanding > 0) {                             // (only reached with requests left when n < 4)
-                mbar_wait(clc_bar(consumed % stages), (consumed / stages) & 1u);
-                ++consumed;
-                --outstanding;
             }
             mbar_wait(empty_bar(s), ph ^ 1u);                     // sentinel: no more tiles
             tile_slot[s] = kDone;
             mbar_arrive(full_bar(s));
+            sched_retire(sched);
         }
     } else {
         // ------------------------------------------------------------ consumers
@@ -508,23 +455,19 @@ vadd_tma_clc(const float* A, const float* B, float* C, size_t n, size_t head, si
             }
             for (; v < nv; v += n_cons)
                 stg128<ST>(cg + v * 4u, add_vec(lds128(sa + v * 16u), lds128(sb + v * 16u)), pol);
-            // the scalar head/tail travel with tile 0, whichever CTA ends up running it (CTA 0 may be
-            // cancelled and its tile taken over under cluster launch control)
-            if (tile == 0) add_edges(A, B, C, n, head, head + nvec4 * 4u, ct);
-
             __syncwarp();
             if ((threadIdx.x & 31u) == 0) mbar_arrive(empty_bar(s));
             if (++s == stages) { s = 0; ph ^= 1u; }
         }
-        // no vector body at all (n < 4 after the head): the grid is the single CTA 0
-        if (body_bytes == 0 && blockIdx.x == 0) add_edges(A, B, C, n, head, head + nvec4 * 4u, ct);
+        // the scalar head/tail: CTA 0 always runs tile 0, and exists even when there is no vector body
+        if (blockIdx.x == 0) add_edges(A, B, C, n, head, head + nvec4 * 4u, ct);
     }
 }
 
 // ---------------------------------------------------------------- ceiling probes
 // The production geometry (512 threads x one 128-bit vector per array) with one side of the
 // traffic removed: what the HBM gives a pure read stream, a pure write stream and a 1:1 copy,
-// next to the add's 2:1 mix (b200va_probe_f32; profiles/r02/README.md section 1a).
+// next to the add's 2:1 mix (b200va_probe_f32).
 __global__ void probe_read2(const float* A, const float* B, float* C, size_t nvec)
 {
     pdl_launch_dependents();

@@ -1,8 +1,8 @@
-// b200va_ptx.cuh -- hand-written PTX primitives for the sm_100a vectorAdd kernels.
+// b200va_ptx.cuh -- hand-written PTX primitives for the sm_90a vectorAdd kernels.
 //
 // Everything here is a thin wrapper over one PTX instruction so that the SASS the
-// kernels produce is predictable (LDG.E.128 / LDG.E.256, UBLKCP, SYNCS.*): no CCCL,
-// no CUTLASS.  Compiled only for -gencode arch=compute_100a,code=sm_100a.
+// kernels produce is predictable (LDG.E.128, UBLKCP, SYNCS.*): no CCCL, no CUTLASS.
+// Compiled only for -gencode arch=compute_90a,code=sm_90a.
 #pragma once
 #include <cstdint>
 
@@ -14,7 +14,7 @@ enum : int {
     LD_PLAIN = 0,   // ld.global
     LD_NA    = 1,   // ld.global.L1::no_allocate               (streaming: skip L1)
     LD_CS    = 2,   // ld.global.cs                             (evict-first streaming)
-    LD_NA_EF = 3,   // L1::no_allocate + L2 evict_first         (policy operand / .L2::evict_first on 256-bit)
+    LD_NA_EF = 3,   // L1::no_allocate + L2 evict_first         (createpolicy operand)
     LD_NC_NA = 4,   // ld.global.nc.L1::no_allocate             (read-only path; NOTE ptxas is then free to
                     //   sink the loads next to their use, which serialises the batch -- kept as a control)
     LD_NA_256 = 5,  // L1::no_allocate + L2::256B prefetch size (SASS LTC256B): L2 fetches 256-B granules
@@ -82,61 +82,21 @@ __device__ __forceinline__ void stg128(float* p, const f32x4& v, uint64_t pol)
                      :: "l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
 }
 
-// ---------------------------------------------------------------- 256-bit global
-// ld/st.global.v8.f32 are new with PTX 8.8 / sm_100 (SASS LDG.E.256 / STG.E.256):
-// one instruction moves a full 32-byte sector per thread, 1 KiB per warp.
+// ---------------------------------------------------------------- 32-byte vectors
+// sm_90 has no 256-bit global access: a 32-byte vector (K3) is two adjacent 128-bit accesses
+// with the same hint, issued back to back, so a warp still moves 1 KiB per instruction pair.
 template <int HINT>
 __device__ __forceinline__ f32x8 ldg256(const float* p, uint64_t pol)
 {
-    f32x8 r;
-    (void)pol;
-    if constexpr (HINT == LD_PLAIN)
-        asm volatile("ld.global.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]),
-                       "=f"(r.v[4]), "=f"(r.v[5]), "=f"(r.v[6]), "=f"(r.v[7]) : "l"(p) : "memory");
-    else if constexpr (HINT == LD_NA)
-        asm volatile("ld.global.L1::no_allocate.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]),
-                       "=f"(r.v[4]), "=f"(r.v[5]), "=f"(r.v[6]), "=f"(r.v[7]) : "l"(p) : "memory");
-    else if constexpr (HINT == LD_NC_NA)
-        asm volatile("ld.global.nc.L1::no_allocate.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]),
-                       "=f"(r.v[4]), "=f"(r.v[5]), "=f"(r.v[6]), "=f"(r.v[7]) : "l"(p) : "memory");
-    else if constexpr (HINT == LD_CS)
-        asm volatile("ld.global.cs.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]),
-                       "=f"(r.v[4]), "=f"(r.v[5]), "=f"(r.v[6]), "=f"(r.v[7]) : "l"(p) : "memory");
-    else if constexpr (HINT == LD_NA_256)
-        asm volatile("ld.global.L1::no_allocate.L2::256B.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]),
-                       "=f"(r.v[4]), "=f"(r.v[5]), "=f"(r.v[6]), "=f"(r.v[7]) : "l"(p) : "memory");
-    else
-        asm volatile("ld.global.L1::no_allocate.L2::evict_first.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]),
-                       "=f"(r.v[4]), "=f"(r.v[5]), "=f"(r.v[6]), "=f"(r.v[7]) : "l"(p) : "memory");
-    return r;
+    const f32x4 lo = ldg128<HINT>(p, pol), hi = ldg128<HINT>(p + 4, pol);
+    return f32x8{{lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w}};
 }
 
 template <int HINT>
 __device__ __forceinline__ void stg256(float* p, const f32x8& r, uint64_t pol)
 {
-    (void)pol;
-    if constexpr (HINT == ST_PLAIN)
-        asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-                     :: "l"(p), "f"(r.v[0]), "f"(r.v[1]), "f"(r.v[2]), "f"(r.v[3]),
-                        "f"(r.v[4]), "f"(r.v[5]), "f"(r.v[6]), "f"(r.v[7]) : "memory");
-    else if constexpr (HINT == ST_NA)
-        asm volatile("st.global.L1::no_allocate.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-                     :: "l"(p), "f"(r.v[0]), "f"(r.v[1]), "f"(r.v[2]), "f"(r.v[3]),
-                        "f"(r.v[4]), "f"(r.v[5]), "f"(r.v[6]), "f"(r.v[7]) : "memory");
-    else if constexpr (HINT == ST_CS)
-        asm volatile("st.global.cs.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-                     :: "l"(p), "f"(r.v[0]), "f"(r.v[1]), "f"(r.v[2]), "f"(r.v[3]),
-                        "f"(r.v[4]), "f"(r.v[5]), "f"(r.v[6]), "f"(r.v[7]) : "memory");
-    else
-        asm volatile("st.global.L1::no_allocate.L2::evict_first.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-                     :: "l"(p), "f"(r.v[0]), "f"(r.v[1]), "f"(r.v[2]), "f"(r.v[3]),
-                        "f"(r.v[4]), "f"(r.v[5]), "f"(r.v[6]), "f"(r.v[7]) : "memory");
+    stg128<HINT>(p, f32x4{r.v[0], r.v[1], r.v[2], r.v[3]}, pol);
+    stg128<HINT>(p + 4, f32x4{r.v[4], r.v[5], r.v[6], r.v[7]}, pol);
 }
 
 // ---------------------------------------------------------------- shared memory
@@ -276,37 +236,25 @@ __device__ __forceinline__ void pdl_wait()
     asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
-// ---------------------------------------------------------------- cluster launch control
-// Blackwell's hardware work-stealing for persistent kernels (PTX 8.6, sm_100): a running
-// CTA asks to cancel the launch of a not-yet-started CTA of the same grid and, on success,
-// receives that CTA's index and does its work.  The 16-byte response lands in shared
-// memory through the async proxy and completes 16 bytes on an mbarrier.
-__device__ __forceinline__ void clc_try_cancel(uint32_t response_smem, uint32_t bar)
+// ---------------------------------------------------------------- dynamic tile scheduler
+// Work stealing for persistent grids: every CTA starts on tile blockIdx.x, then takes tickets
+// from a per-launch counter in global memory (ctr[0]); ticket t is tile gridDim.x + t.  When a
+// CTA has run out of tiles it counts itself out on ctr[1]; the last CTA to do so zeroes both
+// words, so the slot is clean for the next launch that is handed it.  Every access happens
+// after griddepcontrol.wait, i.e. after every earlier launch on the stream has completed.
+__device__ __forceinline__ uint32_t sched_next_tile(unsigned int* ctr)
 {
-    asm volatile("clusterlaunchcontrol.try_cancel.async.shared::cta.mbarrier::complete_tx::bytes.b128 [%0], [%1];"
-                 :: "r"(response_smem), "r"(bar) : "memory");
+    return gridDim.x + atomicAdd(ctr, 1u);
 }
 
-// Decodes a response: returns true and the cancelled CTA's blockIdx.x if the request
-// succeeded; false if there was nothing left to cancel (the index is then undefined).
-__device__ __forceinline__ bool clc_query(uint32_t response_smem, uint32_t& ctaid_x)
+__device__ __forceinline__ void sched_retire(unsigned int* ctr)
 {
-    uint64_t lo, hi;
-    uint32_t ok, x;
-    asm volatile("ld.shared.v2.b64 {%0, %1}, [%2];" : "=l"(lo), "=l"(hi) : "r"(response_smem) : "memory");
-    asm volatile(
-        "{\n"
-        ".reg .b128 resp;\n"
-        ".reg .pred p;\n"
-        "mov.b128 resp, {%2, %3};\n"
-        "clusterlaunchcontrol.query_cancel.is_canceled.pred.b128 p, resp;\n"
-        "selp.b32 %0, 1, 0, p;\n"
-        "mov.b32 %1, 0;\n"
-        "@p clusterlaunchcontrol.query_cancel.get_first_ctaid::x.b32.b128 %1, resp;\n"
-        "}\n"
-        : "=r"(ok), "=r"(x) : "l"(lo), "l"(hi));
-    ctaid_x = x;
-    return ok != 0;
+    __threadfence();                                  // this CTA's last ticket precedes its count
+    if (atomicAdd(ctr + 1, 1u) == gridDim.x - 1) {
+        ctr[0] = 0u;
+        ctr[1] = 0u;
+        __threadfence();
+    }
 }
 
 // Named barrier over a subset of the CTA's warps (id 1..15; 0 is __syncthreads).

@@ -16,7 +16,7 @@
 //                                 (two arrays in, nothing out), fill (one array out), copy (1 in 1 out)
 //                 < geometries.txt
 //
-// Not part of the reference's surface: a development tool for profiles/*.
+// Not part of the reference's surface: a development tool for geometry A/B runs.
 #include <cuda_runtime.h>
 
 #include <algorithm>

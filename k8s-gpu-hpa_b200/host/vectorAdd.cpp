@@ -1,4 +1,4 @@
-// vectorAdd -- the B200-native replacement for the binary the reference runs as
+// vectorAdd -- the H100-native replacement for the binary the reference runs as
 //
 //     image:   "k8s.gcr.io/cuda-vector-add:v0.1"                     cuda-test-deployment.yaml:18
 //     command: for (( c=1; c<=5000; c++ )); do ./vectorAdd; done     cuda-test-deployment.yaml:19
@@ -588,7 +588,7 @@ int run_sharded(const Options& o)
         return EXIT_FAILURE;
     }
     b200va_devinfo_t di;
-    for (int d = 0; d < o.gpus; ++d) va(b200va_query(d, &di), "find a B200-class CUDA device");
+    for (int d = 0; d < o.gpus; ++d) va(b200va_query(d, &di), "find an H100-class CUDA device");
 
     Nvml nvml;
     bool have_nvml = false;
@@ -638,10 +638,10 @@ int run_sharded(const Options& o)
                   "{\"metric\": \"fp32 elements/sec\", \"mode\": \"%s\", \"n\": %zu, \"gpus\": %d, \"kernel\": \"%s\", "
                   "\"iters_per_block\": %d, \"launches_per_gpu\": %lld, \"graph_batch\": %d, \"gpu_ms_max\": %.4f, "
                   "\"ms_per_pass\": %.5f, \"elements_per_s\": %.5e, \"algorithmic_GBps\": %.1f, "
-                  "\"roofline_frac_of_8TBps_per_gpu\": %.4f, \"wall_s\": %.4f, \"gpu_busy_frac\": %.4f, "
+                  "\"roofline_frac_of_3p35TBps_per_gpu\": %.4f, \"wall_s\": %.4f, \"gpu_busy_frac\": %.4f, "
                   "\"mismatches\": %" PRIu64 ", \"digest_sum\": \"%016" PRIx64 "\", \"digest_xor\": \"%08" PRIx64 "\"",
                   o.mode.c_str(), o.n, o.gpus, variant_name(tune.kind), o.iters, launches, o.graph, max_ms,
-                  launches ? max_ms / static_cast<double>(launches) : 0.0, eps, gbps, gbps / (8000.0 * o.gpus), max_wall,
+                  launches ? max_ms / static_cast<double>(launches) : 0.0, eps, gbps, gbps / (3350.0 * o.gpus), max_wall,
                   max_wall > 0 ? max_ms * 1e-3 / max_wall : 0.0, mism, dig[0], dig[1]);
     js = buf;
     if (o.mode == "staged") {

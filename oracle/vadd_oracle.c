@@ -5,7 +5,7 @@
  * and bench.py's cpu_baseline / --impl reference legs may load it.  The product
  * (k8s-gpu-hpa_b200/csrc, the vectorAdd CLI) never links, loads or calls anything here.
  *
- * PARITY UNPINNED BY THE REFERENCE.  /root/reference holds no source and no tests
+ * PARITY UNPINNED BY THE REFERENCE.  The reference repository holds no source and no tests
  * for this path: the arithmetic lives in the third-party container image
  *     k8s.gcr.io/cuda-vector-add:v0.1        (cuda-test-deployment.yaml:18)
  * which the reference only *invokes*:

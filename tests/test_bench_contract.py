@@ -79,7 +79,7 @@ def test_cli_strong_leg_shows_the_executable_exactly_the_ranks_gpus(tmp_path, mo
     fake.write_text("""#!/usr/bin/env python3
 import json, os, sys
 out = sys.argv[sys.argv.index("--json") + 1]
-json.dump({"elements_per_s": 4.7e12, "ms_per_pass": 0.2268, "mismatches": 0, "roofline_frac_of_8TBps_per_gpu": 0.9,
+json.dump({"elements_per_s": 4.7e12, "ms_per_pass": 0.2268, "mismatches": 0, "roofline_frac_of_3p35TBps_per_gpu": 0.9,
            "digest_sum": "0fd8e36879aed49f", "digest_xor": "0f23c595", "seen": os.environ.get("CUDA_VISIBLE_DEVICES"),
            "argv": sys.argv[1:]}, open(out, "w"))
 """)

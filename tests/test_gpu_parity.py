@@ -179,23 +179,24 @@ def test_tuned_geometries_are_all_bit_exact():
                     geos.append(capi.Tune(kind=capi.K2_TMA, threads=threads, ctas_per_sm=1, ld_hint=ld, st_hint=1,
                                           stages=stages, tile_bytes=tile, store_mode=mode))
         geos.append(capi.Tune(kind=capi.K2_TMA, threads=256, ctas_per_sm=2, stages=3, tile_bytes=16384, store_mode=mode))
-    for stages, tile in ((2, 2048), (3, 8192), (4, 8192), (5, 4096), (6, 16384), (4, 28672)):      # CLC tile scheduler
+    for stages, tile in ((2, 2048), (3, 8192), (4, 8192), (5, 4096), (6, 16384), (4, 28672)):      # dynamic tile scheduler
         for threads in (32, 128, 512):
             geos.append(capi.Tune(kind=capi.K2_TMA, threads=threads, ld_hint=0, st_hint=1, stages=stages, tile_bytes=tile,
                                   store_mode=2))
     for threads in (32, 256, 1024):                                  # 4-byte accesses, U loads per array in flight
         for unroll in (4, 8, 16):
             geos.append(capi.Tune(kind=capi.K4_SCALAR_MLP, threads=threads, unroll=unroll))
-    for kind in (capi.K1_VEC128, capi.K3_VEC256):                    # early loads / L2 prefetch and the CLC scheduler (K1c)
+    for kind in (capi.K1_VEC128, capi.K3_VEC256):                    # early loads / L2 prefetch and the dynamic scheduler (K1d)
         for early in (0, 1, 2):
             for unroll in (1, 2, 4, 8):
                 for threads in (64, 256, 512):
                     geos.append(capi.Tune(kind=kind, threads=threads, unroll=unroll, ld_hint=0, st_hint=1, early_loads=early, scheduler=1))
             geos.append(capi.Tune(kind=kind, threads=128, unroll=2, ctas_per_sm=2, ld_hint=3, st_hint=0, early_loads=early))
+    geos.append(capi.Tune(kind=capi.K3_VEC256, threads=1024, unroll=8))
     for t in geos:
         out = torch.full((n,), -1.0, dtype=torch.float32, device="cuda")
-        if t.kind == capi.K4_SCALAR_MLP and t.threads == 1024 and t.unroll == 16:
-            with pytest.raises(pkg.B200VAError) as e:        # 1024 threads x 32 live loads: register-limited, refused
+        if t.kind == capi.K3_VEC256 and t.threads == 1024 and t.unroll == 8:
+            with pytest.raises(pkg.B200VAError) as e:        # 1024 threads x 8 32-byte vectors per array: register-limited, refused
                 va.add(a, b, out, tune=t, full_matrix=True)
             assert e.value.code == capi.ERR_VARIANT
             va.add(a, b, out)                                  # and the refusal leaves no latched CUDA error behind
@@ -214,7 +215,7 @@ def test_tuned_geometries_are_all_bit_exact():
 
 
 def test_production_library_carries_the_production_set_only():
-    """libb200va.so: what AUTO and the named variants resolve to (+ early loads, + K1c) runs; a
+    """libb200va.so: what AUTO and the named variants resolve to (+ early loads, + K1d) runs; a
     geometry only the A/B matrix has is refused with ERR_VARIANT -- and runs in libb200va_tune.so."""
     n = 300_003
     ha, hb = oracle.fill_ctr(n, 0x0A), oracle.fill_ctr(n, 0x0B)
@@ -290,8 +291,9 @@ def test_early_loads_chain_of_launches_is_bit_exact():
 
 
 def test_vec_kernel_under_cluster_launch_control_ragged_sizes_and_offsets():
-    """K1c: the vec tile body with tiles handed out by try_cancel -- every tile exactly once, the
-    scalar head/tail travel with tile 0 whichever CTA runs it."""
+    """K1d, the sm_90a replacement of the cluster-launch-control vec kernel: the vec tile body with
+    tiles handed out by the ticket counter -- every tile exactly once, the scalar head/tail travel
+    with tile 0."""
     nmax = max(SIZES)
     ha, hb = oracle.fill_ctr(nmax + 8, 0x0A, 78), oracle.fill_ctr(nmax + 8, 0x0B, 78)
     a, b = dev(ha), dev(hb)
@@ -303,7 +305,7 @@ def test_vec_kernel_under_cluster_launch_control_ragged_sizes_and_offsets():
                 out = torch.full((n + 16,), -3.0, dtype=torch.float32, device="cuda")
                 va.add(a[off:off + n], b[off:off + n], out[off:off + n], tune=t, full_matrix=True)
                 torch.cuda.synchronize()
-                assert_bits_equal(out[off:off + n], oracle.vadd(ha[off:off + n].copy(), hb[off:off + n].copy()), f"k1c n={n} off={off}")
+                assert_bits_equal(out[off:off + n], oracle.vadd(ha[off:off + n].copy(), hb[off:off + n].copy()), f"k1d n={n} off={off}")
                 assert (out[:off] == -3.0).all() and (out[off + n:] == -3.0).all()
     n = 1 << 24
     x = torch.empty(n, dtype=torch.float32, device="cuda")
@@ -315,14 +317,15 @@ def test_vec_kernel_under_cluster_launch_control_ragged_sizes_and_offsets():
     for _ in range(50):
         va.add(x, y, z, tune=t)
     assert va.digest(z) == oracle.ctr_vadd_digest(n) and va.verify(x, y, z) == (0, -1)
-    # ctas_per_sm (static persistent split) and the CLC scheduler exclude each other
+    # ctas_per_sm (static persistent split) and the dynamic scheduler exclude each other
     with pytest.raises(pkg.B200VAError):
         va.add(x, y, z, tune=capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=2, st_hint=1, scheduler=1, ctas_per_sm=2))
 
 
 def test_clc_scheduled_tma_kernel_ragged_sizes_and_offsets():
-    """store_mode 2: one CTA per tile, resident CTAs steal the rest through cluster launch
-    control -- every tile must be processed exactly once whatever the tile count."""
+    """store_mode 2 (on sm_90a the dynamic tile scheduler takes the place of cluster launch control):
+    a persistent grid whose CTAs claim tiles from the ticket counter -- every tile must be processed
+    exactly once whatever the tile count."""
     nmax = max(SIZES)
     ha, hb = oracle.fill_ctr(nmax + 8, 0x0A, 77), oracle.fill_ctr(nmax + 8, 0x0B, 77)
     a, b = dev(ha), dev(hb)
@@ -334,7 +337,7 @@ def test_clc_scheduled_tma_kernel_ragged_sizes_and_offsets():
                 va.add(a[off:off + n], b[off:off + n], out[off:off + n] if off + n <= n + 16 else out[:n], tune=t)
                 torch.cuda.synchronize()
                 got = out[off:off + n] if off + n <= n + 16 else out[:n]
-                assert_bits_equal(got, oracle.vadd(ha[off:off + n].copy(), hb[off:off + n].copy()), f"clc n={n} off={off}")
+                assert_bits_equal(got, oracle.vadd(ha[off:off + n].copy(), hb[off:off + n].copy()), f"k2d n={n} off={off}")
     # back-to-back launches (PDL chain) keep producing the same bits
     n = 1 << 24
     x = torch.empty(n, dtype=torch.float32, device="cuda")
@@ -415,7 +418,7 @@ def test_device_verify_and_digest_detect_a_single_flipped_bit():
 
 @pytest.mark.parametrize("variant", ["auto", "k1", "k2", "k3"])
 def test_full_size_2p28_properties(variant):
-    """BASELINE.json configs[1]: N = 2^28 on one B200 (3 GiB of operands)."""
+    """BASELINE.json configs[1]: N = 2^28 on one H100 (3 GiB of operands)."""
     n = 1 << 28
     a = torch.empty(n, dtype=torch.float32, device="cuda")
     b = torch.empty_like(a)

@@ -6,17 +6,19 @@ import pytest
 from conftest import ROOT
 from k8s_gpu_hpa_b200 import hpa_replay as hr
 
+GOLD = os.path.join(ROOT, "tests", "golden")
+
 
 def test_constants_match_the_reference_manifests_when_present():
-    ref = "/root/reference"
-    if not os.path.isdir(ref):
-        pytest.skip("reference tree not present on this machine")
-    hpa = open(os.path.join(ref, "cuda-test-hpa.yaml")).read()
-    assert f"targetValue: {int(hr.HPA_TARGET)}" in hpa
-    assert f"minReplicas: {hr.HPA_MIN}" in hpa and f"maxReplicas: {hr.HPA_MAX}" in hpa
-    assert f'"-c", "{int(hr.DCGM_INTERVAL_S * 1000)}"' in open(os.path.join(ref, "dcgm-exporter.yaml")).read().replace("'", '"') \
-        or "10000" in open(os.path.join(ref, "dcgm-exporter.yaml")).read()
-    assert "scrape_interval: 1s" in open(os.path.join(ref, "kube-prometheus-stack-values.yaml")).read()
+    """The manifests' values as extracted into tests/golden/reference_manifests.json
+    (tests/golden/make_reference_command.py)."""
+    import json
+
+    m = json.load(open(os.path.join(GOLD, "reference_manifests.json")))
+    assert m["hpa"]["targetValue"] == hr.HPA_TARGET
+    assert m["hpa"]["minReplicas"] == hr.HPA_MIN and m["hpa"]["maxReplicas"] == hr.HPA_MAX
+    assert m["dcgm_collect_interval_ms"] == hr.DCGM_INTERVAL_S * 1000
+    assert m["scrape_interval"] == f"{hr.SCRAPE_INTERVAL_S:g}s"
 
 
 def test_recording_rule_max_by_pod_then_avg_over_labelled_pods():
@@ -53,8 +55,9 @@ def test_replay_reference_shape_vs_sustained_loop():
 
 @pytest.mark.parametrize("rel", ["r01/aa_hpa_trigger_replay.jsonl", "r02/e_hpa_trigger_replay.jsonl"])
 def test_recorded_gpu_run_replays_to_the_same_decisions(rel):
-    """profiles/r0x/*_hpa_trigger_replay.jsonl: NVML utilisation measured on a B200 while the
-    load generator ran at several duty cycles; the offline rule + HPA must agree with it."""
+    """profiles/r0x/*_hpa_trigger_replay.jsonl (tools/hpa_trigger_replay.py): NVML utilisation measured
+    on an H100 while the load generator ran at several duty cycles; the offline rule + HPA must agree
+    with it."""
     import json
 
     path = os.path.join(ROOT, "profiles", *rel.split("/"))

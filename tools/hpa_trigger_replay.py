@@ -5,7 +5,11 @@ driving GPU utilisation, replayed against the (unchanged) recording rule and HPA
 For each duty-cycle target the drop-in binary runs `--iters 5000`-launch blocks for a
 wall-clock duration while sampling NVML utilisation (the local stand-in for
 dcgm_gpu_utilization); the sampled trace is then fed through hpa_replay.Replay
-(exporter 10 s collect, 1 s scrape, rule, HPA sync 15 s, target 5, 1..3 replicas)."""
+(exporter 10 s collect, 1 s scrape, rule, HPA sync 15 s, target 5, 1..3 replicas).
+
+    python tools/hpa_trigger_replay.py [seconds per target] > profiles/<round>/<name>_hpa_trigger_replay.jsonl
+
+(run on an H100; tests/test_hpa_replay.py replays the committed recordings offline)."""
 import json
 import os
 import subprocess
