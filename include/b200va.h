@@ -161,7 +161,10 @@ int b200va_add_f32_loop(const float *dA, const float *dB, float *dC, size_t n,
 /* Persistent form for a long-running load generator: the graph of `graph_batch` launches
  * is captured once; b200va_loop_run replays it floor(iters/graph_batch) times plus
  * iters%graph_batch direct launches, asynchronously on `stream`.  Destroy only after
- * the stream has drained. */
+ * the stream has drained.  One handle must not be run on two streams at the same time:
+ * every replay of its graph uses the same scratch memory (the ticket counters of the
+ * dynamically scheduled kernels), so two replays in flight at once would share it.
+ * Separate handles are independent. */
 typedef struct b200va_loop b200va_loop_t;
 int b200va_loop_create(b200va_loop_t **out, const float *dA, const float *dB, float *dC,
                        size_t n, int variant, int graph_batch);

@@ -459,11 +459,13 @@ int plan_geometry(const b200va_tune_t& t, const b200va_devinfo_t* di, size_t n, 
     return B200VA_OK;
 }
 
-// Ticket counters of the dynamic tile scheduler: a ring of kSchedSlots two-word slots per device,
-// zeroed once and handed out round-robin, one per launch; the kernel's last CTA zeroes its slot
-// again (b200va_ptx.cuh: sched_retire).  Launches on one stream are ordered (every counter access
-// follows griddepcontrol.wait), so a slot is only ever shared by launches that are kSchedSlots
-// apart in issue order and run concurrently on different streams.
+// Ticket counters of the dynamic tile scheduler for direct launches: a ring of kSchedSlots two-word
+// slots per device, zeroed once and handed out round-robin, one per launch; the kernel's last CTA
+// zeroes its slot again (b200va_ptx.cuh: sched_retire).  Launches on one stream are ordered (every
+// counter access follows griddepcontrol.wait), so a slot is only ever shared by direct launches that
+// are kSchedSlots apart in issue order and run concurrently on different streams.  A captured graph
+// would keep its slots for every replay while the ring moves on and hands them to other launches,
+// so a loop handle's graph takes its counters from the handle instead (b200va_loop::ctr).
 constexpr unsigned kSchedSlots = 4096;
 
 struct SchedPool {
@@ -485,7 +487,7 @@ int sched_slot(int device, unsigned int** out)
         p.ctr = static_cast<unsigned int*>(d);
     });
     if (p.rc != B200VA_OK) return p.rc;
-    if (out) *out = p.ctr + 2 * (p.next.fetch_add(1, std::memory_order_relaxed) % kSchedSlots);
+    *out = p.ctr + 2 * (p.next.fetch_add(1, std::memory_order_relaxed) % kSchedSlots);
     return B200VA_OK;
 }
 
@@ -553,7 +555,10 @@ int check_block_size(Fn fn, unsigned block)
     return block > last_max ? B200VA_ERR_VARIANT : B200VA_OK;
 }
 
-int launch(const float* dA, const float* dB, float* dC, size_t n, b200va_tune_t t, cudaStream_t stream)
+// `ctr`: the dynamic tile scheduler's two-word ticket counter (zeroed; the kernel leaves it zeroed
+// again); nullptr takes the next slot of the device's ring.
+int launch(const float* dA, const float* dB, float* dC, size_t n, b200va_tune_t t, cudaStream_t stream,
+           unsigned int* ctr = nullptr)
 {
     RC_TRY(check_args(dA, dB, dC, n));
     const b200va_devinfo_t* di = nullptr;
@@ -618,8 +623,7 @@ int launch(const float* dA, const float* dB, float* dC, size_t n, b200va_tune_t 
             int resident = 1;
             RC_TRY(resident_ctas(reinterpret_cast<const void*>(fn), g.block, g.smem, &resident));
             RC_TRY(plan_geometry(t, di, n, nvec, resident, &g));
-            unsigned int* ctr = nullptr;
-            RC_TRY(sched_slot(di->device, &ctr));
+            if (!ctr) RC_TRY(sched_slot(di->device, &ctr));
             return launch_kernel(fn, g.grid, g.block, g.smem, stream, dA, dB, dC, n, head, nvec,
                                  static_cast<uint32_t>(t.tile_bytes), static_cast<uint32_t>(t.stages), ctr);
         }
@@ -641,8 +645,7 @@ int launch(const float* dA, const float* dB, float* dC, size_t n, b200va_tune_t 
     int resident = 1;
     RC_TRY(resident_ctas(fn.key(), g.block, 0, &resident));
     RC_TRY(plan_geometry(t, di, n, nvec, resident, &g));
-    unsigned int* ctr = nullptr;
-    RC_TRY(sched_slot(di->device, &ctr));
+    if (!ctr) RC_TRY(sched_slot(di->device, &ctr));
     return launch_kernel(fn.dyn, g.grid, g.block, 0, stream, dA, dB, dC, n, head, nvec, g.ntiles, ctr);
 }
 
@@ -865,6 +868,9 @@ struct b200va_loop {
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     bool pdl_edges = false;
+    // ticket counters of the graph's nodes (two words per node) when the tune is dynamically
+    // scheduled: owned by the handle, so no other launch can be handed them while the graph replays
+    unsigned int* ctr = nullptr;
 };
 
 static int capture_batch(b200va_loop* l, cudaStream_t cap)
@@ -875,7 +881,8 @@ static int capture_batch(b200va_loop* l, cudaStream_t cap)
     // so their loads may run ahead of the dependency (launch() drops the hint if C aliases A or B)
     b200va_tune_t follow = l->tune;
     follow.early_loads = 1;
-    for (int i = 0; i < l->batch && rc == B200VA_OK; ++i) rc = launch(l->dA, l->dB, l->dC, l->n, i ? follow : l->tune, cap);
+    for (int i = 0; i < l->batch && rc == B200VA_OK; ++i)
+        rc = launch(l->dA, l->dB, l->dC, l->n, i ? follow : l->tune, cap, l->ctr ? l->ctr + 2 * i : nullptr);
     cudaGraph_t g = nullptr;
     const cudaError_t e = cudaStreamEndCapture(cap, &g);
     if (rc != B200VA_OK || e != cudaSuccess) {
@@ -896,6 +903,7 @@ int b200va_loop_destroy(b200va_loop_t* l)
     if (!l) return B200VA_OK;
     if (l->exec) cudaGraphExecDestroy(l->exec);
     if (l->graph) cudaGraphDestroy(l->graph);
+    if (l->ctr) cudaFree(l->ctr);
     delete l;
     return B200VA_OK;
 }
@@ -914,23 +922,34 @@ int b200va_loop_create(b200va_loop_t** out, const float* dA, const float* dB, fl
     default_tune(variant, n, &l->tune);
     cudaError_t e = cudaGetDevice(&l->device);
     if (e != cudaSuccess) { delete l; return cuda_err(e); }
-    if (l->tune.scheduler == 1 || (l->tune.kind == B200VA_K2_TMA && l->tune.store_mode == 2)) {
-        const int rc = sched_slot(l->device, nullptr);    // allocate the ticket counters before any capture
-        if (rc != B200VA_OK) { delete l; return rc; }
-    }
     if (l->batch > 1 && n > 0) {
         cudaStream_t cap = nullptr;
         e = cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking);
         if (e != cudaSuccess) { delete l; return cuda_err(e); }
+        if (l->tune.scheduler == 1 || (l->tune.kind == B200VA_K2_TMA && l->tune.store_mode == 2)) {
+            const size_t bytes = static_cast<size_t>(l->batch) * 2 * sizeof(unsigned int);
+            void* d = nullptr;
+            e = cudaMalloc(&d, bytes);
+            l->ctr = static_cast<unsigned int*>(d);
+            if (e == cudaSuccess) e = cudaMemsetAsync(d, 0, bytes, cap);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(cap);   // zero before the first replay, on any stream
+            if (e != cudaSuccess) {
+                cudaGetLastError();
+                cudaStreamDestroy(cap);
+                b200va_loop_destroy(l);
+                return cuda_err(e);
+            }
+        }
         int rc = capture_batch(l, cap);
         l->pdl_edges = (rc == B200VA_OK) && pdl_enabled();
-        if (rc != B200VA_OK && pdl_enabled()) {   // older drivers: capture without programmatic edges
+        // older drivers: capture without programmatic edges (same counters: a failed capture ran nothing)
+        if (rc != B200VA_OK && pdl_enabled()) {
             tl_pdl_off = true;
             rc = capture_batch(l, cap);
             tl_pdl_off = false;
         }
         cudaStreamDestroy(cap);
-        if (rc != B200VA_OK) { delete l; return rc; }
+        if (rc != B200VA_OK) { b200va_loop_destroy(l); return rc; }
     }
     *out = l;
     return B200VA_OK;

@@ -290,67 +290,6 @@ def test_early_loads_chain_of_launches_is_bit_exact():
     assert capi.lib.b200va_add_f32_ex(x.data_ptr(), x.data_ptr(), x.data_ptr(), n, 0, 0x80, None) == capi.ERR_INVALID
 
 
-def test_vec_kernel_under_cluster_launch_control_ragged_sizes_and_offsets():
-    """K1d, the sm_90a replacement of the cluster-launch-control vec kernel: the vec tile body with
-    tiles handed out by the ticket counter -- every tile exactly once, the scalar head/tail travel
-    with tile 0."""
-    nmax = max(SIZES)
-    ha, hb = oracle.fill_ctr(nmax + 8, 0x0A, 78), oracle.fill_ctr(nmax + 8, 0x0B, 78)
-    a, b = dev(ha), dev(hb)
-    for t in (capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=2, st_hint=1, scheduler=1),
-              capi.Tune(kind=capi.K1_VEC128, threads=64, unroll=4, st_hint=1, scheduler=1, early_loads=1),
-              capi.Tune(kind=capi.K3_VEC256, threads=32, unroll=1, st_hint=1, scheduler=1)):
-        for n in SIZES:
-            for off in (0, 1, 3):
-                out = torch.full((n + 16,), -3.0, dtype=torch.float32, device="cuda")
-                va.add(a[off:off + n], b[off:off + n], out[off:off + n], tune=t, full_matrix=True)
-                torch.cuda.synchronize()
-                assert_bits_equal(out[off:off + n], oracle.vadd(ha[off:off + n].copy(), hb[off:off + n].copy()), f"k1d n={n} off={off}")
-                assert (out[:off] == -3.0).all() and (out[off + n:] == -3.0).all()
-    n = 1 << 24
-    x = torch.empty(n, dtype=torch.float32, device="cuda")
-    y = torch.empty_like(x)
-    z = torch.empty_like(x)
-    va.fill_ctr(x, 0x0A)
-    va.fill_ctr(y, 0x0B)
-    t = capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=2, st_hint=1, scheduler=1, early_loads=1)
-    for _ in range(50):
-        va.add(x, y, z, tune=t)
-    assert va.digest(z) == oracle.ctr_vadd_digest(n) and va.verify(x, y, z) == (0, -1)
-    # ctas_per_sm (static persistent split) and the dynamic scheduler exclude each other
-    with pytest.raises(pkg.B200VAError):
-        va.add(x, y, z, tune=capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=2, st_hint=1, scheduler=1, ctas_per_sm=2))
-
-
-def test_clc_scheduled_tma_kernel_ragged_sizes_and_offsets():
-    """store_mode 2 (on sm_90a the dynamic tile scheduler takes the place of cluster launch control):
-    a persistent grid whose CTAs claim tiles from the ticket counter -- every tile must be processed
-    exactly once whatever the tile count."""
-    nmax = max(SIZES)
-    ha, hb = oracle.fill_ctr(nmax + 8, 0x0A, 77), oracle.fill_ctr(nmax + 8, 0x0B, 77)
-    a, b = dev(ha), dev(hb)
-    for t in (capi.Tune(kind=capi.K2_TMA, threads=128, st_hint=1, stages=4, tile_bytes=8192, store_mode=2),
-              capi.Tune(kind=capi.K2_TMA, threads=64, st_hint=0, stages=3, tile_bytes=2048, store_mode=2)):
-        for n in SIZES:
-            for off in (0, 1, 3):
-                out = torch.full((n + 16,), -3.0, dtype=torch.float32, device="cuda")
-                va.add(a[off:off + n], b[off:off + n], out[off:off + n] if off + n <= n + 16 else out[:n], tune=t)
-                torch.cuda.synchronize()
-                got = out[off:off + n] if off + n <= n + 16 else out[:n]
-                assert_bits_equal(got, oracle.vadd(ha[off:off + n].copy(), hb[off:off + n].copy()), f"k2d n={n} off={off}")
-    # back-to-back launches (PDL chain) keep producing the same bits
-    n = 1 << 24
-    x = torch.empty(n, dtype=torch.float32, device="cuda")
-    y = torch.empty_like(x)
-    z = torch.empty_like(x)
-    va.fill_ctr(x, 0x0A)
-    va.fill_ctr(y, 0x0B)
-    t = capi.Tune(kind=capi.K2_TMA, threads=128, st_hint=1, stages=4, tile_bytes=8192, store_mode=2)
-    for _ in range(50):
-        va.add(x, y, z, tune=t)
-    assert va.digest(z) == oracle.ctr_vadd_digest(n) and va.verify(x, y, z) == (0, -1)
-
-
 @pytest.mark.parametrize("n", [0, 1, 3, 4, 5, 1023, 1 << 16, (1 << 20) + 3, 7_000_001])
 def test_support_kernels_vector_and_scalar_paths_agree(n):
     """fill_ctr / verify / digest have a 128-bit form for 16-byte-aligned pointers and a scalar one otherwise:
@@ -492,32 +431,39 @@ def test_beyond_32_bit_indexing_n_2p32_plus():
 
 
 def test_launch_loop_matches_single_launch_with_and_without_graphs():
+    """Every variant, in the one-shot loop and a persistent loop handle.  C is poisoned (a finite 0x7F byte pattern)
+    before every run and checked after it: every launch of a run writes the same C, so only a fresh pattern shows a
+    launch that left part of C unwritten."""
+    import ctypes as C
+
     n = 1 << 22
     a = torch.empty(n, dtype=torch.float32, device="cuda")
     b = torch.empty_like(a)
     va.fill_ctr(a, 0x0A)
     va.fill_ctr(b, 0x0B)
     want = oracle.ctr_vadd_digest(n)
+    c = torch.empty_like(a)
     s = torch.cuda.Stream()
-    with torch.cuda.stream(s):
-        for iters, batch in ((1, 0), (7, 0), (50, 10), (53, 10), (5, 8)):
-            c = torch.zeros_like(a)
-            va.add_loop(a, b, c, iters, graph_batch=batch)
+    for variant in ALL:
+        with torch.cuda.stream(s):
+            for iters, batch in ((1, 0), (7, 0), (50, 10), (53, 10), (5, 8)):
+                c.view(torch.int32).fill_(0x7F7F7F7F)
+                va.add_loop(a, b, c, iters, graph_batch=batch, variant=variant)
+                s.synchronize()
+                assert va.digest(c) == want, (variant, iters, batch)
+        # the legacy default stream is fine too: the batch is captured on a private stream
+        c.view(torch.int32).fill_(0x7F7F7F7F)
+        rc = capi.lib.b200va_add_f32_loop(a.data_ptr(), b.data_ptr(), c.data_ptr(), n, capi.VARIANTS[variant], 20, 10, None)
+        assert rc == capi.OK
+        torch.cuda.synchronize()
+        assert va.digest(c) == want, variant
+        # persistent loop handle: one capture, many replays
+        h = C.c_void_p()
+        assert capi.lib.b200va_loop_create(C.byref(h), a.data_ptr(), b.data_ptr(), c.data_ptr(), n, capi.VARIANTS[variant], 16) == capi.OK
+        for iters in (16, 40, 3, 16):
+            with torch.cuda.stream(s):
+                c.view(torch.int32).fill_(0x7F7F7F7F)
+            assert capi.lib.b200va_loop_run(h, iters, s.cuda_stream) == capi.OK
             s.synchronize()
-            assert va.digest(c) == want, (iters, batch)
-    # the legacy default stream is fine too: the batch is captured on a private stream
-    c = torch.zeros_like(a)
-    rc = capi.lib.b200va_add_f32_loop(a.data_ptr(), b.data_ptr(), c.data_ptr(), n, 0, 20, 10, None)
-    assert rc == capi.OK
-    torch.cuda.synchronize()
-    assert va.digest(c) == want
-    # persistent loop handle: one capture, many replays
-    import ctypes as C
-    h = C.c_void_p()
-    c = torch.zeros_like(a)
-    assert capi.lib.b200va_loop_create(C.byref(h), a.data_ptr(), b.data_ptr(), c.data_ptr(), n, 0, 16) == capi.OK
-    for iters in (16, 40, 3):
-        assert capi.lib.b200va_loop_run(h, iters, s.cuda_stream) == capi.OK
-    s.synchronize()
-    assert capi.lib.b200va_loop_destroy(h) == capi.OK
-    assert va.digest(c) == want
+            assert va.digest(c) == want, (variant, iters)
+        assert capi.lib.b200va_loop_destroy(h) == capi.OK
