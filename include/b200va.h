@@ -117,8 +117,10 @@ int         b200va_query(int device, b200va_devinfo_t *out);
 int         b200va_resolve(int variant, size_t n, b200va_tune_t *out);
 int         b200va_resolve_ex(int variant, size_t n, unsigned flags, b200va_tune_t *out);
 
-/* Launch geometry a tune resolves to on `device` for n elements with 32-byte-aligned
- * pointers (what "CUDA kernel launch with %d blocks of %d threads" prints, a5). */
+/* Launch geometry of b200va_add_f32_tuned(tune) on `device` for n elements with distinct,
+ * 256-byte-aligned pointers (what "CUDA kernel launch with %d blocks of %d threads" prints,
+ * a5).  Planned exactly as that call plans its launch: for a tune it would launch, the
+ * geometry it launches with; for a tune it refuses, its error code. */
 int         b200va_geometry(const b200va_tune_t *tune, size_t n, int device,
                             unsigned *grid, unsigned *block, unsigned *dyn_smem_bytes);
 

@@ -17,7 +17,9 @@
 #include <cctype>
 #include <condition_variable>
 #include <functional>
+#include <map>
 #include <thread>
+#include <utility>
 #include <vector>
 #include <cstdio>
 #include <cstdlib>
@@ -122,7 +124,6 @@ using dyn_fn = void (*)(const float*, const float*, float*, size_t, size_t, size
 struct VecFn {
     vec_fn plain = nullptr;
     dyn_fn dyn = nullptr;
-    explicit operator bool() const { return plain || dyn; }
     const void* key() const { return plain ? reinterpret_cast<const void*>(plain) : reinterpret_cast<const void*>(dyn); }
 };
 
@@ -268,27 +269,6 @@ tma_fn pick_tma(int store_mode, bool l2_hint, int st)
 #endif
 }
 
-std::mutex g_attr_mu;
-
-// Opt in to > 48 KiB dynamic shared memory once per (function, device).
-int ensure_smem_optin(const void* fn, int device, int bytes)
-{
-    struct Key { const void* fn; int device; int bytes; };
-    static Key seen[256];
-    static int n_seen = 0;
-    std::lock_guard<std::mutex> lk(g_attr_mu);
-    for (int i = 0; i < n_seen; ++i)
-        if (seen[i].fn == fn && seen[i].device == device) {
-            if (seen[i].bytes >= bytes) return B200VA_OK;
-            CU_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-            seen[i].bytes = bytes;
-            return B200VA_OK;
-        }
-    CU_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-    if (n_seen < 256) seen[n_seen++] = Key{fn, device, bytes};
-    return B200VA_OK;
-}
-
 // ----------------------------------------------------------------------- geometry
 // Production choices per size class.  K_AUTO is always the 128-bit kernel; thread count / unroll /
 // cache hints follow the footprint (12 n bytes) AND what the caller says about the data:
@@ -379,6 +359,34 @@ void default_tune(int variant, size_t n, b200va_tune_t* t, unsigned flags = 0)
     }
 }
 
+// The named variants and B200VA_F_* hints the entry points accept.
+int check_variant(int variant, unsigned flags = 0)
+{
+    if (variant < B200VA_K_AUTO || variant > B200VA_K3_VEC256) return B200VA_ERR_VARIANT;
+    return (flags & ~(B200VA_F_INPUTS_STABLE | B200VA_F_COLD)) ? B200VA_ERR_INVALID : B200VA_OK;
+}
+
+// The tune b200va_add_f32_tuned runs for `in`: K_AUTO takes the whole AUTO tune for n, other zero
+// fields the defaults of the tune's kind.
+int complete_tune(const b200va_tune_t& in, size_t n, b200va_tune_t* out)
+{
+    b200va_tune_t t = in;
+    b200va_tune_t d;
+    default_tune(t.kind, n, &d);
+    if (t.kind == B200VA_K_AUTO) t = d;
+    if (t.kind == B200VA_K4_SCALAR_MLP) {
+        if (t.threads == 0) t.threads = 256;
+        if (t.unroll == 0) t.unroll = 8;
+    }
+    if (t.threads == 0) t.threads = d.threads;
+    if (t.unroll == 0) t.unroll = d.unroll ? d.unroll : 1;
+    if (t.stages == 0) t.stages = d.stages;
+    if (t.tile_bytes == 0) t.tile_bytes = d.tile_bytes;
+    if (t.early_loads < 0 || t.early_loads > 2 || (t.scheduler & ~1)) return B200VA_ERR_VARIANT;
+    *out = t;
+    return B200VA_OK;
+}
+
 inline bool is_pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
 
 int check_args(const float* dA, const float* dB, const float* dC, size_t n)
@@ -395,67 +403,86 @@ int check_args(const float* dA, const float* dB, const float* dC, size_t n)
     return B200VA_OK;
 }
 
-// Launch geometry of a (validated) tune for a vector body of `nvec` vectors: the single
-// place grid/block/smem are computed -- used by launch() and reported by b200va_geometry().
-struct Geometry {
+// ----------------------------------------------------------------------- launch plan
+// The kernel forms of an add: the scalar control K0, the 4-byte kernel K4, the vec kernels of K1/K3 under
+// the block scheduler or the dynamic tile scheduler (K1d), K2's TMA ring with a static or dynamic (K2d) split.
+enum class Form { Scalar, K4, Vec, VecDyn, Tma, TmaDyn };
+
+using scalar_fn = void (*)(const float*, const float*, float*, size_t);
+
+// One launch as plan_launch decides it: run by launch(), reported by b200va_geometry().
+struct Plan {
+    Form form = Form::Scalar;
+    scalar_fn scalar = nullptr;      // Scalar, K4
+    VecFn vec;                       // Vec, VecDyn
+    tma_fn tma = nullptr;
+    tma_dyn_fn tma_dyn = nullptr;
     unsigned grid = 1, block = 0;
-    size_t smem = 0, ntiles = 0;
+    size_t smem = 0, head = 0, nvec = 0, ntiles = 0;   // Scalar, K4: a tile is one CTA's threads x unroll elements
+    bool ctr = false;                // dynamically scheduled: takes a two-word ticket counter
 };
 
-// `resident`: CTAs of the selected kernel that fit on one SM at once (the occupancy calculator's
-// answer); it sizes the persistent grid of the dynamic tile scheduler.
-int plan_geometry(const b200va_tune_t& t, const b200va_devinfo_t* di, size_t n, size_t nvec, int resident, Geometry* g)
+// Validates the tune for the plan's form and sets block, dynamic shared memory and tile count.
+int plan_block(const b200va_tune_t& t, const b200va_devinfo_t* di, size_t n, Plan* p)
 {
-    if (t.kind == B200VA_K0_SCALAR) {
-        const size_t blocks = (n + 255) / 256;
-        if (blocks > 0x7fffffffull) return B200VA_ERR_INVALID;
-        g->grid = static_cast<unsigned>(blocks ? blocks : 1);
-        g->block = 256;
-        return B200VA_OK;
-    }
-    if (t.kind == B200VA_K2_TMA) {
-        if (t.threads < 32 || t.threads > 992 || (t.threads & 31)) return B200VA_ERR_VARIANT;
-        if (t.stages < 2 || t.stages > 32) return B200VA_ERR_VARIANT;
-        if (t.tile_bytes < 2048 || (t.tile_bytes & 2047)) return B200VA_ERR_VARIANT;
-        if (t.st_hint < 0 || t.st_hint >= ST_HINTS) return B200VA_ERR_VARIANT;
-        if (t.store_mode < 0 || t.store_mode > 2) return B200VA_ERR_VARIANT;
-        // ring + full/empty barriers; the dynamic-scheduler form adds a tile slot per stage
-        const long long smem = static_cast<long long>(t.stages) * 2 * t.tile_bytes +
-                               (t.store_mode == 2 ? 20LL : 16LL) * t.stages;
-        if (smem > di->max_smem_optin) return B200VA_ERR_VARIANT;
-        g->smem = static_cast<size_t>(smem);
-        g->ntiles = (nvec * 16u + t.tile_bytes - 1) / t.tile_bytes;
-        size_t grid = static_cast<size_t>(di->sm_count) * (t.ctas_per_sm > 0 ? t.ctas_per_sm : 1);
-        if (t.store_mode == 2) {                          // persistent: every CTA that fits at once, tiles by ticket
-            if (g->ntiles > 0x7fffffffull) return B200VA_ERR_INVALID;
-            grid = static_cast<size_t>(di->sm_count) * static_cast<size_t>(resident > 0 ? resident : 1);
-        }
-        if (grid > 0x7fffffffull) return B200VA_ERR_INVALID;
-        if (grid > g->ntiles) grid = g->ntiles;
-        g->grid = static_cast<unsigned>(grid ? grid : 1);
-        g->block = static_cast<unsigned>(t.threads + 32);     // + the producer warp
-        return B200VA_OK;
-    }
-    if (t.kind != B200VA_K1_VEC128 && t.kind != B200VA_K3_VEC256) return B200VA_ERR_VARIANT;
     if (t.threads < 32 || t.threads > 1024 || (t.threads & 31)) return B200VA_ERR_VARIANT;
-    if (!is_pow2(t.unroll) || t.unroll > 8) return B200VA_ERR_VARIANT;
-    if (t.ld_hint < 0 || t.ld_hint >= LD_HINTS || t.st_hint < 0 || t.st_hint >= ST_HINTS) return B200VA_ERR_VARIANT;
-    if (t.scheduler < 0 || t.scheduler > 1 || (t.scheduler == 1 && t.ctas_per_sm != 0)) return B200VA_ERR_VARIANT;
-    const size_t tile_vecs = static_cast<size_t>(t.threads) * t.unroll;
-    g->ntiles = (nvec + tile_vecs - 1) / tile_vecs;
-    size_t grid = g->ntiles;
-    if (t.scheduler == 1) {                               // persistent grid, 32-bit tile index
+    p->block = static_cast<unsigned>(t.threads);
+    switch (p->form) {
+        case Form::K4:
+            if (t.unroll != 4 && t.unroll != 8 && t.unroll != 16) return B200VA_ERR_VARIANT;
+            [[fallthrough]];
+        case Form::Scalar: {
+            const size_t per_cta = static_cast<size_t>(t.threads) * t.unroll;
+            p->ntiles = (n + per_cta - 1) / per_cta;
+            break;
+        }
+        case Form::Tma:
+        case Form::TmaDyn: {
+            if (t.threads > 992 || t.stages < 2 || t.stages > 32) return B200VA_ERR_VARIANT;
+            if (t.tile_bytes < 2048 || (t.tile_bytes & 2047)) return B200VA_ERR_VARIANT;
+            if (t.st_hint < 0 || t.st_hint >= ST_HINTS) return B200VA_ERR_VARIANT;
+            if (t.store_mode < 0 || t.store_mode > 2) return B200VA_ERR_VARIANT;
+            // ring + full/empty barriers; the dynamic-scheduler form adds a tile slot per stage
+            const long long smem = static_cast<long long>(t.stages) * 2 * t.tile_bytes +
+                                   (t.store_mode == 2 ? 20LL : 16LL) * t.stages;
+            if (smem > di->max_smem_optin) return B200VA_ERR_VARIANT;
+            p->smem = static_cast<size_t>(smem);
+            p->ntiles = (p->nvec * 16u + t.tile_bytes - 1) / t.tile_bytes;
+            p->block += 32;                                   // + the producer warp
+            break;
+        }
+        case Form::Vec:
+        case Form::VecDyn: {
+            if (!is_pow2(t.unroll) || t.unroll > 8) return B200VA_ERR_VARIANT;
+            if (t.ld_hint < 0 || t.ld_hint >= LD_HINTS || t.st_hint < 0 || t.st_hint >= ST_HINTS) return B200VA_ERR_VARIANT;
+            if (t.scheduler < 0 || t.scheduler > 1 || (t.scheduler == 1 && t.ctas_per_sm != 0)) return B200VA_ERR_VARIANT;
+            const size_t tile_vecs = static_cast<size_t>(t.threads) * t.unroll;
+            p->ntiles = (p->nvec + tile_vecs - 1) / tile_vecs;
+            break;
+        }
+    }
+    if (p->ctr && p->ntiles > 0x7fffffffull) return B200VA_ERR_INVALID;   // 32-bit tile tickets
+    return B200VA_OK;
+}
+
+// The grid: one CTA per tile, capped for the persistent forms at the CTAs that fit at once --
+// `resident` per SM (the occupancy calculator's answer) under the dynamic scheduler, else ctas_per_sm.
+int plan_grid(const b200va_tune_t& t, const b200va_devinfo_t* di, int resident, Plan* p)
+{
+    const size_t sms = static_cast<size_t>(di->sm_count);
+    size_t grid = p->ntiles;
+    if (p->form == Form::Tma || p->form == Form::TmaDyn) {
+        grid = sms * static_cast<size_t>(p->ctr ? resident : t.ctas_per_sm > 0 ? t.ctas_per_sm : 1);
         if (grid > 0x7fffffffull) return B200VA_ERR_INVALID;
-        const size_t cap = static_cast<size_t>(di->sm_count) * static_cast<size_t>(resident > 0 ? resident : 1);
-        if (grid > cap) grid = cap;
+        if (grid > p->ntiles) grid = p->ntiles;
+    } else if (p->form == Form::Vec || p->form == Form::VecDyn) {
+        if (p->ctr && grid > sms * resident) grid = sms * resident;
+        if (t.ctas_per_sm > 0 && grid > sms * t.ctas_per_sm) grid = sms * t.ctas_per_sm;
+        if (grid > 0x7fffffffull) grid = 0x7fffffffull;   // the kernel loops tile += gridDim.x
+    } else if (grid > 0x7fffffffull) {
+        return B200VA_ERR_INVALID;
     }
-    if (t.ctas_per_sm > 0) {
-        const size_t cap = static_cast<size_t>(di->sm_count) * t.ctas_per_sm;
-        if (grid > cap) grid = cap;
-    }
-    if (grid > 0x7fffffffull) grid = 0x7fffffffull;   // the kernel loops tile += gridDim.x
-    g->grid = static_cast<unsigned>(grid ? grid : 1);
-    g->block = static_cast<unsigned>(t.threads);
+    p->grid = static_cast<unsigned>(grid ? grid : 1);
     return B200VA_OK;
 }
 
@@ -491,38 +518,142 @@ int sched_slot(int device, unsigned int** out)
     return B200VA_OK;
 }
 
-// CTAs of `fn` (block threads, smem dynamic bytes) that are resident on one SM at once.
-int resident_ctas(const void* fn, unsigned block, size_t smem, int* out)
+// The runtime's answers about one kernel on one device.
+struct KernelAttrs {
+    int max_block = 0, smem_optin = 0, resident = 0;
+    unsigned res_block = 0;
+    size_t res_smem = 0;
+};
+std::mutex g_attr_mu;
+std::map<std::pair<const void*, int>, KernelAttrs> g_attrs;
+
+// Refuses a CTA larger than `fn` runs (register-limited for the deep unrolls), opts in to `smem` bytes of
+// dynamic shared memory and, given `resident`, returns the CTAs of this shape resident on one SM at once
+// (cached for the last shape asked).  A cached answer makes no CUDA call.
+int kernel_attrs(const void* fn, int device, unsigned block, size_t smem, int* resident)
 {
-    thread_local const void* last_fn = nullptr;
-    thread_local unsigned last_block = 0;
-    thread_local size_t last_smem = 0;
-    thread_local int last = 0;
-    if (fn != last_fn || block != last_block || smem != last_smem) {
-        int k = 0;
-        CU_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k, fn, static_cast<int>(block), smem));
-        last_fn = fn; last_block = block; last_smem = smem; last = k;
+    std::lock_guard<std::mutex> lk(g_attr_mu);
+    KernelAttrs* k = nullptr;
+    try {
+        k = &g_attrs[{fn, device}];
+    } catch (...) {
+        return B200VA_ERR_NOMEM;
     }
-    *out = last > 0 ? last : 1;
+    if (k->max_block == 0) {
+        cudaFuncAttributes fa;
+        CU_TRY(cudaFuncGetAttributes(&fa, fn));
+        k->max_block = fa.maxThreadsPerBlock;
+    }
+    if (block > static_cast<unsigned>(k->max_block)) return B200VA_ERR_VARIANT;
+    if (smem > static_cast<size_t>(k->smem_optin)) {
+        CU_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+        k->smem_optin = static_cast<int>(smem);
+    }
+    if (resident) {
+        if (k->resident == 0 || k->res_block != block || k->res_smem != smem) {
+            int r = 0;
+            CU_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, fn, static_cast<int>(block), smem));
+            k->resident = r > 0 ? r : 1;
+            k->res_block = block;
+            k->res_smem = smem;
+        }
+        *resident = k->resident;
+    }
     return B200VA_OK;
 }
 
-// All hot-path launches go through here: programmatic stream serialization lets launch
-// k+1 ramp up behind launch k's tail (the kernels call griddepcontrol.wait before their
-// first global access, so stream order is unchanged).  B200VA_NO_PDL=1 disables it.
-thread_local bool tl_pdl_off = false;   // set while re-capturing a graph without PDL edges
+// The one place an add kernel and its geometry are decided, for C = A + B at these addresses (never
+// dereferenced).  Each step runs once: alias rules, vector width and head peel, tune validation, kernel
+// pick, register limit, shared-memory opt-in, occupancy, grid.
+int plan_launch(b200va_tune_t t, const b200va_devinfo_t* di, const void* pa, const void* pb, const void* pc, size_t n,
+                Plan* p)
+{
+    const uintptr_t a = reinterpret_cast<uintptr_t>(pa), b = reinterpret_cast<uintptr_t>(pb),
+                    c = reinterpret_cast<uintptr_t>(pc);
+    if (a == c || b == c) {
+        // .nc (non-coherent) loads require data that is read-only for the kernel's lifetime
+        if (t.ld_hint == LD_NC_NA) t.ld_hint = LD_PLAIN;
+        // early register loads (1) read A and B while the previous launch may still be running: the
+        // always-legal L2 prefetch (2) takes their place
+        if (t.early_loads == 1) t.early_loads = 2;
+    }
 
+    int vw = 0;
+    if (t.kind == B200VA_K3_VEC256) vw = 8;
+    else if (t.kind == B200VA_K1_VEC128 || t.kind == B200VA_K2_TMA) vw = 4;
+    else if (t.kind != B200VA_K0_SCALAR && t.kind != B200VA_K4_SCALAR_MLP) return B200VA_ERR_VARIANT;
+    // vector body needs A, B, C equally misaligned w.r.t. the vector width (K3 falls back to 16 bytes)
+    for (; vw; vw = vw == 8 ? 4 : 0) {
+        const uintptr_t mask = static_cast<uintptr_t>(vw) * 4u - 1u;
+        if ((a & mask) == (b & mask) && (a & mask) == (c & mask)) {
+            p->head = ((static_cast<uintptr_t>(vw) * 4u - (a & mask)) & mask) / 4u;
+            break;
+        }
+    }
+    if (p->head > n) p->head = n;
+    if (vw) p->nvec = (n - p->head) / static_cast<size_t>(vw);
+    if (t.kind == B200VA_K0_SCALAR) {
+        p->form = Form::Scalar;
+        t.threads = 256;                  // the sample's launch shape
+        t.unroll = 1;
+    } else if (vw == 0) {
+        // the explicit K4 variant, and the path taken when A, B, C share no 16-byte phase (no vector
+        // body exists): 256 threads x 8 loads per array in flight
+        if (t.kind != B200VA_K4_SCALAR_MLP) { t.threads = 256; t.unroll = 8; }
+        p->form = Form::K4;
+    } else if (t.kind == B200VA_K2_TMA) {
+        p->form = t.store_mode == 2 ? Form::TmaDyn : Form::Tma;
+    } else {
+        p->form = t.scheduler == 1 ? Form::VecDyn : Form::Vec;
+    }
+    p->ctr = p->form == Form::VecDyn || p->form == Form::TmaDyn;
+
+    RC_TRY(plan_block(t, di, n, p));
+
+    const void* fn = nullptr;
+    switch (p->form) {
+        case Form::Scalar:
+        case Form::K4:
+            p->scalar = p->form == Form::Scalar ? vadd_scalar : t.unroll == 4 ? vadd_scalar_unrolled<4>
+                      : t.unroll == 8 ? vadd_scalar_unrolled<8> : vadd_scalar_unrolled<16>;
+            fn = reinterpret_cast<const void*>(p->scalar);
+            break;
+        case Form::Vec:
+        case Form::VecDyn:
+            p->vec = pick_vec(vw, t.unroll, t.ld_hint, t.st_hint, t.early_loads, t.scheduler);
+            fn = p->vec.key();
+            break;
+        case Form::Tma:
+            p->tma = pick_tma(t.store_mode, t.ld_hint == LD_NA_EF, t.st_hint);
+            fn = reinterpret_cast<const void*>(p->tma);
+            break;
+        case Form::TmaDyn:
+            p->tma_dyn = pick_tma_dyn(t.ld_hint == LD_NA_EF, t.st_hint);
+            fn = reinterpret_cast<const void*>(p->tma_dyn);
+            break;
+    }
+    if (!fn) return B200VA_ERR_VARIANT;   // not compiled into this library
+    // CTAs of up to 256 threads are never register-limited (255 registers per thread fit)
+    int resident = 1;
+    if (p->block > 256 || p->smem || p->ctr)
+        RC_TRY(kernel_attrs(fn, di->device, p->block, p->smem, p->ctr ? &resident : nullptr));
+    return plan_grid(t, di, resident, p);
+}
+
+// Programmatic stream serialization lets launch k+1 ramp up behind launch k's tail (the kernels
+// call griddepcontrol.wait before their first global access, so stream order is unchanged).  Every
+// hot-path launch uses it unless B200VA_NO_PDL=1.
 bool pdl_enabled()
 {
     static const bool on = [] {
         const char* e = std::getenv("B200VA_NO_PDL");
         return !(e && e[0] == '1');
     }();
-    return on && !tl_pdl_off;
+    return on;
 }
 
 template <class... KArgs, class... Args>
-int launch_kernel(void (*fn)(KArgs...), unsigned grid, unsigned block, size_t smem, cudaStream_t stream, Args... args)
+int launch_kernel(void (*fn)(KArgs...), unsigned grid, unsigned block, size_t smem, cudaStream_t stream, bool pdl, Args... args)
 {
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid);
@@ -533,120 +664,55 @@ int launch_kernel(void (*fn)(KArgs...), unsigned grid, unsigned block, size_t sm
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = pdl ? 1 : 0;
     const cudaError_t e = cudaLaunchKernelEx(&cfg, fn, static_cast<KArgs>(args)...);
     if (e != cudaSuccess) cudaGetLastError();   // a refused launch must not stay latched for the next caller
     return cuda_err(e);
 }
 
-// Largest CTA the kernel can be launched with (register-limited for the deep unrolls).
-template <class Fn>
-int check_block_size(Fn fn, unsigned block)
-{
-    thread_local const void* last_fn = nullptr;
-    thread_local unsigned last_max = 0;
-    const void* key = reinterpret_cast<const void*>(fn);
-    if (key != last_fn) {
-        cudaFuncAttributes fa;
-        CU_TRY(cudaFuncGetAttributes(&fa, key));
-        last_fn = key;
-        last_max = static_cast<unsigned>(fa.maxThreadsPerBlock);
-    }
-    return block > last_max ? B200VA_ERR_VARIANT : B200VA_OK;
-}
-
 // `ctr`: the dynamic tile scheduler's two-word ticket counter (zeroed; the kernel leaves it zeroed
 // again); nullptr takes the next slot of the device's ring.
-int launch(const float* dA, const float* dB, float* dC, size_t n, b200va_tune_t t, cudaStream_t stream,
+int launch(const float* dA, const float* dB, float* dC, size_t n, const b200va_tune_t& t, cudaStream_t stream, bool pdl,
            unsigned int* ctr = nullptr)
 {
     RC_TRY(check_args(dA, dB, dC, n));
     const b200va_devinfo_t* di = nullptr;
     RC_TRY(current_dev_info(&di));
     if (n == 0) return B200VA_OK;
-
-    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), b = reinterpret_cast<uintptr_t>(dB),
-                    c = reinterpret_cast<uintptr_t>(dC);
-    const bool aliased = (a == c) || (b == c);
-    // .nc (non-coherent) loads require data that is read-only for the kernel's lifetime
-    if (aliased && t.ld_hint == LD_NC_NA) t.ld_hint = LD_PLAIN;
-
-    int vw = 0;
-    if (t.kind == B200VA_K3_VEC256) vw = 8;
-    else if (t.kind == B200VA_K1_VEC128 || t.kind == B200VA_K2_TMA) vw = 4;
-    else if (t.kind != B200VA_K0_SCALAR && t.kind != B200VA_K4_SCALAR_MLP) return B200VA_ERR_VARIANT;
-
-    // vector body needs A, B, C equally misaligned w.r.t. the vector width
-    size_t head = 0;
-    while (vw) {
-        const uintptr_t mask = static_cast<uintptr_t>(vw) * 4u - 1u;
-        if ((a & mask) == (b & mask) && (a & mask) == (c & mask)) {
-            head = ((static_cast<uintptr_t>(vw) * 4u - (a & mask)) & mask) / 4u;
-            break;
-        }
-        if (t.kind == B200VA_K2_TMA) { vw = 0; break; }
-        vw = (vw == 8) ? 4 : 0;
+    Plan p;
+    RC_TRY(plan_launch(t, di, dA, dB, dC, n, &p));
+    if (p.ctr && !ctr) RC_TRY(sched_slot(di->device, &ctr));
+    const uint32_t tile = static_cast<uint32_t>(t.tile_bytes), stages = static_cast<uint32_t>(t.stages);
+    switch (p.form) {
+        case Form::Scalar:   // the control keeps the sample's plain launch (no programmatic dependent launch)
+            p.scalar<<<p.grid, p.block, 0, stream>>>(dA, dB, dC, n);
+            return cuda_err(cudaGetLastError());
+        case Form::K4:
+            return launch_kernel(p.scalar, p.grid, p.block, 0, stream, pdl, dA, dB, dC, n);
+        case Form::Vec:
+            return launch_kernel(p.vec.plain, p.grid, p.block, 0, stream, pdl, dA, dB, dC, n, p.head, p.nvec, p.ntiles);
+        case Form::VecDyn:
+            return launch_kernel(p.vec.dyn, p.grid, p.block, 0, stream, pdl, dA, dB, dC, n, p.head, p.nvec, p.ntiles, ctr);
+        case Form::Tma:
+            return launch_kernel(p.tma, p.grid, p.block, p.smem, stream, pdl, dA, dB, dC, n, p.head, p.nvec, tile, stages);
+        case Form::TmaDyn:
+            return launch_kernel(p.tma_dyn, p.grid, p.block, p.smem, stream, pdl, dA, dB, dC, n, p.head, p.nvec, tile,
+                                 stages, ctr);
     }
-    Geometry g;
-    if (t.kind == B200VA_K4_SCALAR_MLP || (vw == 0 && t.kind != B200VA_K0_SCALAR)) {
-        // 4-byte kernel with U loads per array per thread in flight: explicit A/B variant, and the
-        // path taken when A, B, C share no 16-byte phase (no vector body exists)
-        const bool explicit_geo = t.kind == B200VA_K4_SCALAR_MLP;
-        const unsigned threads = explicit_geo ? static_cast<unsigned>(t.threads) : 256u;
-        const int U = explicit_geo ? t.unroll : 8;
-        if (threads < 32 || threads > 1024 || (threads & 31u)) return B200VA_ERR_VARIANT;
-        if (U != 4 && U != 8 && U != 16) return B200VA_ERR_VARIANT;
-        const size_t per_cta = static_cast<size_t>(threads) * static_cast<size_t>(U);
-        const size_t blocks = (n + per_cta - 1) / per_cta;
-        if (blocks > 0x7fffffffull) return B200VA_ERR_INVALID;
-        auto fn = U == 4 ? vadd_scalar_unrolled<4> : U == 8 ? vadd_scalar_unrolled<8> : vadd_scalar_unrolled<16>;
-        if (threads > 256) RC_TRY(check_block_size(fn, threads));
-        return launch_kernel(fn, static_cast<unsigned>(blocks), threads, 0, stream, dA, dB, dC, n);
-    }
-    if (vw == 0) {  // the scalar control
-        b200va_tune_t k0{};
-        k0.kind = B200VA_K0_SCALAR;
-        RC_TRY(plan_geometry(k0, di, n, 0, 1, &g));
-        // the control keeps the sample's plain launch (no programmatic dependent launch)
-        vadd_scalar<<<g.grid, g.block, 0, stream>>>(dA, dB, dC, n);
-        return cuda_err(cudaGetLastError());
-    }
-    if (head > n) head = n;
-    const size_t nvec = (n - head) / static_cast<size_t>(vw);
+    return B200VA_ERR_VARIANT;
+}
 
-    if (t.kind == B200VA_K2_TMA) {
-        if (t.store_mode == 2) {
-            tma_dyn_fn fn = pick_tma_dyn(t.ld_hint == LD_NA_EF, t.st_hint);
-            if (!fn) return B200VA_ERR_VARIANT;
-            RC_TRY(plan_geometry(t, di, n, nvec, 1, &g));     // validates the tune and sizes the ring
-            RC_TRY(ensure_smem_optin(reinterpret_cast<const void*>(fn), di->device, static_cast<int>(g.smem)));
-            int resident = 1;
-            RC_TRY(resident_ctas(reinterpret_cast<const void*>(fn), g.block, g.smem, &resident));
-            RC_TRY(plan_geometry(t, di, n, nvec, resident, &g));
-            if (!ctr) RC_TRY(sched_slot(di->device, &ctr));
-            return launch_kernel(fn, g.grid, g.block, g.smem, stream, dA, dB, dC, n, head, nvec,
-                                 static_cast<uint32_t>(t.tile_bytes), static_cast<uint32_t>(t.stages), ctr);
-        }
-        RC_TRY(plan_geometry(t, di, n, nvec, 1, &g));
-        tma_fn fn = pick_tma(t.store_mode, t.ld_hint == LD_NA_EF, t.st_hint);
-        if (!fn) return B200VA_ERR_VARIANT;
-        RC_TRY(ensure_smem_optin(reinterpret_cast<const void*>(fn), di->device, static_cast<int>(g.smem)));
-        return launch_kernel(fn, g.grid, g.block, g.smem, stream, dA, dB, dC, n, head, nvec,
-                             static_cast<uint32_t>(t.tile_bytes), static_cast<uint32_t>(t.stages));
-    }
-    // early register loads (1) read A and B while the previous launch may still be running: never when C aliases
-    // an input -- the always-legal L2 prefetch (2) takes their place
-    const int early = (t.early_loads == 1 && aliased) ? 2 : t.early_loads;
-    RC_TRY(plan_geometry(t, di, n, nvec, 1, &g));             // validates the tune before a kernel is picked
-    const VecFn fn = pick_vec(vw, t.unroll, t.ld_hint, t.st_hint, early, t.scheduler);
-    if (!fn) return B200VA_ERR_VARIANT;
-    if (g.block > 256) RC_TRY(check_block_size(fn.key(), g.block));   // deep unrolls: the CTA size is register-limited
-    if (fn.plain) return launch_kernel(fn.plain, g.grid, g.block, 0, stream, dA, dB, dC, n, head, nvec, g.ntiles);
-    int resident = 1;
-    RC_TRY(resident_ctas(fn.key(), g.block, 0, &resident));
-    RC_TRY(plan_geometry(t, di, n, nvec, resident, &g));
-    if (!ctr) RC_TRY(sched_slot(di->device, &ctr));
-    return launch_kernel(fn.dyn, g.grid, g.block, 0, stream, dA, dB, dC, n, head, nvec, g.ntiles, ctr);
+// `count` launches of the same add on `stream`.  One that follows what the caller queued runs `t`; one
+// that follows the same add (`after_same` for the first), which writes only C, runs with early_loads = 1.
+// `ctr`, if set, gives launch i the ticket counter at ctr + 2 i instead of a ring slot.
+int launch_chain(const float* dA, const float* dB, float* dC, size_t n, const b200va_tune_t& t, bool after_same,
+                 int count, cudaStream_t stream, bool pdl, unsigned int* ctr = nullptr)
+{
+    b200va_tune_t follow = t;
+    follow.early_loads = 1;
+    for (int i = 0; i < count; ++i)
+        RC_TRY(launch(dA, dB, dC, n, i || after_same ? follow : t, stream, pdl, ctr ? ctr + 2 * i : nullptr));
+    return B200VA_OK;
 }
 
 unsigned support_grid(const b200va_devinfo_t* di, size_t n, int threads)
@@ -724,7 +790,7 @@ int launch_stream_typed(const void* dA, const void* dB, void* dC, size_t n, doub
         if (skip_l1_stores) fn = unroll == 2 ? stream_vec<DT, OP, 2, LD_PLAIN, ST_NA> : stream_vec<DT, OP, 1, LD_PLAIN, ST_NA>;
         else fn = unroll == 2 ? stream_vec<DT, OP, 2, LD_PLAIN, ST_PLAIN> : stream_vec<DT, OP, 1, LD_PLAIN, ST_PLAIN>;
     }
-    return launch_kernel(fn, static_cast<unsigned>(grid), threads, 0, st, dA, dB, dC, n, head, nvec, ntiles, s, prefetch_first);
+    return launch_kernel(fn, static_cast<unsigned>(grid), threads, 0, st, pdl_enabled(), dA, dB, dC, n, head, nvec, ntiles, s, prefetch_first);
 }
 
 template <int DT>
@@ -779,15 +845,13 @@ int b200va_query(int device, b200va_devinfo_t* out)
 
 int b200va_resolve(int variant, size_t n, b200va_tune_t* out)
 {
-    if (!out || variant < B200VA_K_AUTO || variant > B200VA_K3_VEC256) return B200VA_ERR_VARIANT;
-    default_tune(variant, n, out);
-    return B200VA_OK;
+    return b200va_resolve_ex(variant, n, 0, out);
 }
 
 int b200va_resolve_ex(int variant, size_t n, unsigned flags, b200va_tune_t* out)
 {
-    if (!out || variant < B200VA_K_AUTO || variant > B200VA_K3_VEC256) return B200VA_ERR_VARIANT;
-    if (flags & ~(B200VA_F_INPUTS_STABLE | B200VA_F_COLD)) return B200VA_ERR_INVALID;
+    if (!out) return B200VA_ERR_VARIANT;
+    RC_TRY(check_variant(variant, flags));
     default_tune(variant, n, out, flags);
     return B200VA_OK;
 }
@@ -798,63 +862,40 @@ int b200va_geometry(const b200va_tune_t* tune, size_t n, int device, unsigned* g
     if (!tune || !grid || !block) return B200VA_ERR_INVALID;
     const b200va_devinfo_t* di = nullptr;
     RC_TRY(dev_info(device, &di));
-    Geometry g;
-    const size_t vw = tune->kind == B200VA_K3_VEC256 ? 8 : 4;
-    RC_TRY(plan_geometry(*tune, di, n, n / vw, 1, &g));
-    const void* dyn = nullptr;                    // the dynamic scheduler's grid depends on the kernel's occupancy
-    if (tune->kind == B200VA_K2_TMA && tune->store_mode == 2)
-        dyn = reinterpret_cast<const void*>(pick_tma_dyn(tune->ld_hint == LD_NA_EF, tune->st_hint));
-    else if ((tune->kind == B200VA_K1_VEC128 || tune->kind == B200VA_K3_VEC256) && tune->scheduler == 1)
-        dyn = pick_vec(static_cast<int>(vw), tune->unroll, tune->ld_hint, tune->st_hint, tune->early_loads, 1).key();
-    if (dyn) {
-        DeviceGuard guard(device);
-        CU_TRY(guard.err);
-        if (g.smem) RC_TRY(ensure_smem_optin(dyn, device, static_cast<int>(g.smem)));
-        int resident = 1;
-        RC_TRY(resident_ctas(dyn, g.block, g.smem, &resident));
-        RC_TRY(plan_geometry(*tune, di, n, n / vw, resident, &g));
-    }
-    *grid = g.grid;
-    *block = g.block;
-    if (dyn_smem_bytes) *dyn_smem_bytes = static_cast<unsigned>(g.smem);
+    b200va_tune_t t;
+    RC_TRY(complete_tune(*tune, n, &t));
+    DeviceGuard guard(device);
+    CU_TRY(guard.err);
+    // notional operands, distinct and 256-byte aligned: the plan reads only their values
+    const float* base = reinterpret_cast<const float*>(uintptr_t{256});
+    Plan p;
+    RC_TRY(plan_launch(t, di, base, base + 64, base + 128, n, &p));
+    *grid = p.grid;
+    *block = p.block;
+    if (dyn_smem_bytes) *dyn_smem_bytes = static_cast<unsigned>(p.smem);
     return B200VA_OK;
 }
 
 int b200va_add_f32(const float* dA, const float* dB, float* dC, size_t n, int variant, void* stream)
 {
-    if (variant < B200VA_K_AUTO || variant > B200VA_K3_VEC256) return B200VA_ERR_VARIANT;
-    b200va_tune_t t;
-    default_tune(variant, n, &t);
-    return launch(dA, dB, dC, n, t, static_cast<cudaStream_t>(stream));
+    return b200va_add_f32_ex(dA, dB, dC, n, variant, 0, stream);
 }
 
 int b200va_add_f32_ex(const float* dA, const float* dB, float* dC, size_t n, int variant, unsigned flags, void* stream)
 {
-    if (variant < B200VA_K_AUTO || variant > B200VA_K3_VEC256) return B200VA_ERR_VARIANT;
-    if (flags & ~(B200VA_F_INPUTS_STABLE | B200VA_F_COLD)) return B200VA_ERR_INVALID;
+    RC_TRY(check_variant(variant, flags));
     b200va_tune_t t;
     default_tune(variant, n, &t, flags);
-    return launch(dA, dB, dC, n, t, static_cast<cudaStream_t>(stream));
+    return launch(dA, dB, dC, n, t, static_cast<cudaStream_t>(stream), pdl_enabled());
 }
 
 int b200va_add_f32_tuned(const float* dA, const float* dB, float* dC, size_t n,
                          const b200va_tune_t* tune, void* stream)
 {
     if (!tune) return B200VA_ERR_INVALID;
-    b200va_tune_t t = *tune;
-    b200va_tune_t d;
-    default_tune(t.kind, n, &d);
-    if (t.kind == B200VA_K_AUTO) t = d;
-    if (t.kind == B200VA_K4_SCALAR_MLP) {
-        if (t.threads == 0) t.threads = 256;
-        if (t.unroll == 0) t.unroll = 8;
-    }
-    if (t.threads == 0) t.threads = d.threads;
-    if (t.unroll == 0) t.unroll = d.unroll ? d.unroll : 1;
-    if (t.stages == 0) t.stages = d.stages;
-    if (t.tile_bytes == 0) t.tile_bytes = d.tile_bytes;
-    if (t.early_loads < 0 || t.early_loads > 2 || (t.scheduler & ~1)) return B200VA_ERR_VARIANT;
-    return launch(dA, dB, dC, n, t, static_cast<cudaStream_t>(stream));
+    b200va_tune_t t;
+    RC_TRY(complete_tune(*tune, n, &t));
+    return launch(dA, dB, dC, n, t, static_cast<cudaStream_t>(stream), pdl_enabled());
 }
 
 // ---- a1: the launch loop --------------------------------------------------------------
@@ -867,22 +908,16 @@ struct b200va_loop {
     int device = 0;
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
-    bool pdl_edges = false;
     // ticket counters of the graph's nodes (two words per node) when the tune is dynamically
     // scheduled: owned by the handle, so no other launch can be handed them while the graph replays
     unsigned int* ctr = nullptr;
 };
 
-static int capture_batch(b200va_loop* l, cudaStream_t cap)
+static int capture_batch(b200va_loop* l, cudaStream_t cap, bool pdl)
 {
     CU_TRY(cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal));
-    int rc = B200VA_OK;
-    // node 0 follows an unknown predecessor; nodes 1.. follow the same add (which writes only C),
-    // so their loads may run ahead of the dependency (launch() drops the hint if C aliases A or B)
-    b200va_tune_t follow = l->tune;
-    follow.early_loads = 1;
-    for (int i = 0; i < l->batch && rc == B200VA_OK; ++i)
-        rc = launch(l->dA, l->dB, l->dC, l->n, i ? follow : l->tune, cap, l->ctr ? l->ctr + 2 * i : nullptr);
+    // node 0 follows an unknown predecessor
+    const int rc = launch_chain(l->dA, l->dB, l->dC, l->n, l->tune, false, l->batch, cap, pdl, l->ctr);
     cudaGraph_t g = nullptr;
     const cudaError_t e = cudaStreamEndCapture(cap, &g);
     if (rc != B200VA_OK || e != cudaSuccess) {
@@ -896,6 +931,33 @@ static int capture_batch(b200va_loop* l, cudaStream_t cap)
     l->graph = g;
     l->exec = x;
     return B200VA_OK;
+}
+
+// The handle's device, counters and graph.  A failure leaves what was made to b200va_loop_destroy.
+static int loop_init(b200va_loop* l)
+{
+    CU_TRY(cudaGetDevice(&l->device));
+    if (l->batch <= 1 || l->n == 0) return B200VA_OK;
+    cudaStream_t cap = nullptr;
+    CU_TRY(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
+    cudaError_t e = cudaSuccess;
+    if (l->tune.scheduler == 1 || (l->tune.kind == B200VA_K2_TMA && l->tune.store_mode == 2)) {
+        const size_t bytes = static_cast<size_t>(l->batch) * 2 * sizeof(unsigned int);
+        void* d = nullptr;
+        e = cudaMalloc(&d, bytes);
+        l->ctr = static_cast<unsigned int*>(d);
+        if (e == cudaSuccess) e = cudaMemsetAsync(d, 0, bytes, cap);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(cap);   // zero before the first replay, on any stream
+        if (e != cudaSuccess) cudaGetLastError();
+    }
+    int rc = cuda_err(e);
+    if (rc == B200VA_OK) {
+        rc = capture_batch(l, cap, pdl_enabled());
+        // older drivers: capture without programmatic edges (same counters: a failed capture ran nothing)
+        if (rc != B200VA_OK && pdl_enabled()) rc = capture_batch(l, cap, false);
+    }
+    cudaStreamDestroy(cap);
+    return rc;
 }
 
 int b200va_loop_destroy(b200va_loop_t* l)
@@ -913,44 +975,15 @@ int b200va_loop_create(b200va_loop_t** out, const float* dA, const float* dB, fl
 {
     if (!out || graph_batch < 0) return B200VA_ERR_INVALID;
     *out = nullptr;
-    if (variant < B200VA_K_AUTO || variant > B200VA_K3_VEC256) return B200VA_ERR_VARIANT;
+    RC_TRY(check_variant(variant));
     RC_TRY(check_args(dA, dB, dC, n));
     b200va_loop* l = new (std::nothrow) b200va_loop;
     if (!l) return B200VA_ERR_NOMEM;
     l->dA = dA; l->dB = dB; l->dC = dC; l->n = n;
     l->batch = graph_batch > 1 ? graph_batch : 1;
     default_tune(variant, n, &l->tune);
-    cudaError_t e = cudaGetDevice(&l->device);
-    if (e != cudaSuccess) { delete l; return cuda_err(e); }
-    if (l->batch > 1 && n > 0) {
-        cudaStream_t cap = nullptr;
-        e = cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking);
-        if (e != cudaSuccess) { delete l; return cuda_err(e); }
-        if (l->tune.scheduler == 1 || (l->tune.kind == B200VA_K2_TMA && l->tune.store_mode == 2)) {
-            const size_t bytes = static_cast<size_t>(l->batch) * 2 * sizeof(unsigned int);
-            void* d = nullptr;
-            e = cudaMalloc(&d, bytes);
-            l->ctr = static_cast<unsigned int*>(d);
-            if (e == cudaSuccess) e = cudaMemsetAsync(d, 0, bytes, cap);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(cap);   // zero before the first replay, on any stream
-            if (e != cudaSuccess) {
-                cudaGetLastError();
-                cudaStreamDestroy(cap);
-                b200va_loop_destroy(l);
-                return cuda_err(e);
-            }
-        }
-        int rc = capture_batch(l, cap);
-        l->pdl_edges = (rc == B200VA_OK) && pdl_enabled();
-        // older drivers: capture without programmatic edges (same counters: a failed capture ran nothing)
-        if (rc != B200VA_OK && pdl_enabled()) {
-            tl_pdl_off = true;
-            rc = capture_batch(l, cap);
-            tl_pdl_off = false;
-        }
-        cudaStreamDestroy(cap);
-        if (rc != B200VA_OK) { b200va_loop_destroy(l); return rc; }
-    }
+    const int rc = loop_init(l);
+    if (rc != B200VA_OK) { b200va_loop_destroy(l); return rc; }
     *out = l;
     return B200VA_OK;
 }
@@ -960,29 +993,22 @@ int b200va_loop_run(b200va_loop_t* l, int iters, void* stream)
     if (!l || iters < 0) return B200VA_ERR_INVALID;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     int left = iters;
-    bool first = true;                       // the first launch of a run follows whatever the caller queued before
-    if (l->exec) {
-        for (; left >= l->batch; left -= l->batch) { CU_TRY(cudaGraphLaunch(l->exec, st)); first = false; }
-    }
-    b200va_tune_t follow = l->tune;
-    follow.early_loads = 1;
-    for (; left > 0; --left) { RC_TRY(launch(l->dA, l->dB, l->dC, l->n, first ? l->tune : follow, st)); first = false; }
-    return B200VA_OK;
+    if (l->exec)
+        for (; left >= l->batch; left -= l->batch) CU_TRY(cudaGraphLaunch(l->exec, st));
+    // the rest are direct launches; the first follows whatever the caller queued unless a replay ran
+    return launch_chain(l->dA, l->dB, l->dC, l->n, l->tune, left < iters, left, st, pdl_enabled());
 }
 
 int b200va_add_f32_loop(const float* dA, const float* dB, float* dC, size_t n, int variant, int iters,
                         int graph_batch, void* stream)
 {
     if (iters < 0 || graph_batch < 0) return B200VA_ERR_INVALID;
-    if (variant < B200VA_K_AUTO || variant > B200VA_K3_VEC256) return B200VA_ERR_VARIANT;
+    RC_TRY(check_variant(variant));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (graph_batch <= 1 || iters < graph_batch) {
-        b200va_tune_t t, follow;
+        b200va_tune_t t;
         default_tune(variant, n, &t);
-        follow = t;
-        follow.early_loads = 1;
-        for (int i = 0; i < iters; ++i) RC_TRY(launch(dA, dB, dC, n, i ? follow : t, st));
-        return B200VA_OK;
+        return launch_chain(dA, dB, dC, n, t, false, iters, st, pdl_enabled());
     }
     b200va_loop_t* l = nullptr;
     RC_TRY(b200va_loop_create(&l, dA, dB, dC, n, variant, graph_batch));
@@ -1127,9 +1153,9 @@ int b200va_probe_f32(int kind, const float* dA, const float* dB, float* dC, size
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const unsigned grid = static_cast<unsigned>(blocks);
     switch (kind) {
-        case B200VA_PROBE_READ2: return launch_kernel(probe_read2, grid, 512u, 0, st, dA, dB, dC, nvec);
-        case B200VA_PROBE_FILL:  return launch_kernel(probe_fill, grid, 512u, 0, st, dC, nvec, 1.0f);
-        default:                 return launch_kernel(probe_copy, grid, 512u, 0, st, dA, dC, nvec);
+        case B200VA_PROBE_READ2: return launch_kernel(probe_read2, grid, 512u, 0, st, pdl_enabled(), dA, dB, dC, nvec);
+        case B200VA_PROBE_FILL:  return launch_kernel(probe_fill, grid, 512u, 0, st, pdl_enabled(), dC, nvec, 1.0f);
+        default:                 return launch_kernel(probe_copy, grid, 512u, 0, st, pdl_enabled(), dA, dC, nvec);
     }
 }
 
@@ -1483,7 +1509,7 @@ static int stage_zero_copy(b200va_stager* s, const float* hA, const float* hB, f
     }
     b200va_tune_t t;
     default_tune(variant == B200VA_K_AUTO ? B200VA_K1_VEC128 : variant, n, &t);
-    return launch(dA, dB, dC, n, t, s->main);
+    return launch(dA, dB, dC, n, t, s->main, pdl_enabled());
 }
 
 static int stage_slots(b200va_stager* s, const float* hA, const float* hB, float* hC, size_t n, int variant)
@@ -1501,7 +1527,7 @@ static int stage_slots(b200va_stager* s, const float* hA, const float* hB, float
         CU_TRY(cudaMemcpyAsync(dA, hA + off, m * sizeof(float), cudaMemcpyHostToDevice, s->slot[i]));
         CU_TRY(cudaMemcpyAsync(dB, hB + off, m * sizeof(float), cudaMemcpyHostToDevice, s->slot[i]));
         default_tune(variant, m, &t, B200VA_F_COLD);      // a chunk fresh off the copy engine is never in L2
-        RC_TRY(launch(dA, dB, dC, m, t, s->slot[i]));
+        RC_TRY(launch(dA, dB, dC, m, t, s->slot[i], pdl_enabled()));
         CU_TRY(cudaMemcpyAsync(hC + off, dC, m * sizeof(float), cudaMemcpyDeviceToHost, s->slot[i]));
     }
     for (int i = 0; i < s->depth; ++i) {
@@ -1552,7 +1578,7 @@ static int stage_lanes(b200va_stager* s, const float* hA, const float* hB, float
         if (inject_fault_at_chunk(k)) return B200VA_ERR_INVALID;   // test hook: fail with copies in flight
         CU_TRY(cudaStreamWaitEvent(s->lane_k, s->ev_in[i], 0));
         default_tune(variant, m, &t, B200VA_F_COLD);      // a chunk fresh off the copy engine is never in L2
-        RC_TRY(launch(dA, dB, dC, m, t, s->lane_k));
+        RC_TRY(launch(dA, dB, dC, m, t, s->lane_k, pdl_enabled()));
         CU_TRY(cudaEventRecord(s->ev_sum[i], s->lane_k));
         CU_TRY(cudaStreamWaitEvent(s->lane_d2h, s->ev_sum[i], 0));
         CU_TRY(cudaMemcpyAsync(hC + off, dC, m * sizeof(float), cudaMemcpyDeviceToHost, s->lane_d2h));
@@ -1602,7 +1628,7 @@ static int stage_bounce(b200va_stager* s, const float* hA, const float* hB, floa
             CU_TRY(cudaEventRecord(s->ev_in[i], s->lane_h2d));
             CU_TRY(cudaStreamWaitEvent(s->lane_k, s->ev_in[i], 0));
             default_tune(variant, m, &t, B200VA_F_COLD);
-            RC_TRY(launch(dA, dA + s->chunk, dA + 2 * s->chunk, m, t, s->lane_k));
+            RC_TRY(launch(dA, dA + s->chunk, dA + 2 * s->chunk, m, t, s->lane_k, pdl_enabled()));
             CU_TRY(cudaEventRecord(s->ev_sum[i], s->lane_k));
             CU_TRY(cudaStreamWaitEvent(s->lane_d2h, s->ev_sum[i], 0));
             CU_TRY(cudaMemcpyAsync(pA + 2 * bc, dA + 2 * s->chunk, m * sizeof(float), cudaMemcpyDeviceToHost, s->lane_d2h));
@@ -1678,7 +1704,7 @@ int b200va_stager_add_f32(b200va_stager_t* s, const float* hA, const float* hB, 
                           int variant, int mode)
 {
     if (!s || (n && (!hA || !hB || !hC))) return B200VA_ERR_INVALID;
-    if (variant < B200VA_K_AUTO || variant > B200VA_K3_VEC256) return B200VA_ERR_VARIANT;
+    RC_TRY(check_variant(variant));
     if (mode < B200VA_STAGE_AUTO || mode > B200VA_STAGE_REGISTER) return B200VA_ERR_INVALID;
     DeviceGuard guard(s->device);
     CU_TRY(guard.err);

@@ -7,8 +7,10 @@ shards): through size-independent properties -- the order-independent digest of 
 result equals the oracle's digest of A+B (a checksum of checksums over shards), the
 device-side recompute finds no mismatch, commutativity, idempotence, in-place == out-of-place.
 """
+import ctypes as C
 import json
 import os
+import re
 
 import numpy as np
 import pytest
@@ -37,6 +39,13 @@ def assert_bits_equal(got, want: np.ndarray, what=""):
     g = got.cpu().numpy() if not isinstance(got, np.ndarray) else got
     bad = oracle.first_mismatch(g, want)
     assert bad < 0, f"{what}: first mismatch at {bad}: got {g.view(np.uint32)[bad]:08x} want {want.view(np.uint32)[bad]:08x}"
+
+
+def geometry(t, n, lib=None):
+    """b200va_geometry for tune t at n elements on the current device: (return code, grid, block)."""
+    grid, block = C.c_uint(), C.c_uint()
+    rc = (lib or capi.lib).b200va_geometry(C.byref(t), n, torch.cuda.current_device(), C.byref(grid), C.byref(block), None)
+    return rc, grid.value, block.value
 
 
 @pytest.mark.parametrize("variant", ALL)
@@ -195,10 +204,11 @@ def test_tuned_geometries_are_all_bit_exact():
     geos.append(capi.Tune(kind=capi.K3_VEC256, threads=1024, unroll=8))
     for t in geos:
         out = torch.full((n,), -1.0, dtype=torch.float32, device="cuda")
+        geo_rc = geometry(t, n, capi.tune_lib())[0]           # b200va_geometry refuses exactly what the launch refuses
         if t.kind == capi.K3_VEC256 and t.threads == 1024 and t.unroll == 8:
             with pytest.raises(pkg.B200VAError) as e:        # 1024 threads x 8 32-byte vectors per array: register-limited, refused
                 va.add(a, b, out, tune=t, full_matrix=True)
-            assert e.value.code == capi.ERR_VARIANT
+            assert e.value.code == capi.ERR_VARIANT and geo_rc == capi.ERR_VARIANT
             va.add(a, b, out)                                  # and the refusal leaves no latched CUDA error behind
             torch.cuda.synchronize()
             assert_bits_equal(out, want, "after refused launch")
@@ -209,35 +219,87 @@ def test_tuned_geometries_are_all_bit_exact():
             # register-limited CTA sizes are refused up front (ERR_VARIANT), never fail at launch
             live = t.threads * t.unroll * (2 if t.kind == capi.K3_VEC256 else 1)
             assert e.code == capi.ERR_VARIANT and t.kind in (capi.K1_VEC128, capi.K3_VEC256) and live >= 8192, t.as_dict()
+            assert geo_rc == e.code, t.as_dict()
             continue
+        assert geo_rc == capi.OK, t.as_dict()
         torch.cuda.synchronize()
         assert_bits_equal(out, want, str(t.as_dict()))
 
 
+PRODUCTION_SIZES = (1 << 10, 1 << 20, 1 << 21, 1 << 22, 1 << 23, 1 << 24, 1 << 28)
+
+
+def production_tunes():
+    """(size, tune): what AUTO and the named variants resolve to for each size class and hint."""
+    return [(size, pkg.resolve(v, size, flags)) for size in PRODUCTION_SIZES for v in pkg.VARIANTS.values()
+            for flags in (0, capi.F_INPUTS_STABLE, capi.F_COLD, capi.F_COLD | capi.F_INPUTS_STABLE)]
+
+
+def k1d_tunes():
+    """The K1d (dynamic tile scheduler) tunes the production library carries."""
+    return (capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=2, st_hint=1, scheduler=1),
+            capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=4, st_hint=1, scheduler=1, early_loads=1))
+
+
 def test_production_library_carries_the_production_set_only():
     """libb200va.so: what AUTO and the named variants resolve to (+ early loads, + K1d) runs; a
-    geometry only the A/B matrix has is refused with ERR_VARIANT -- and runs in libb200va_tune.so."""
+    geometry only the A/B matrix has is refused with ERR_VARIANT -- and runs in libb200va_tune.so.
+    b200va_geometry of the same library answers for exactly the tunes that run."""
     n = 300_003
     ha, hb = oracle.fill_ctr(n, 0x0A), oracle.fill_ctr(n, 0x0B)
     want = oracle.vadd(ha, hb)
     a, b = dev(ha), dev(hb)
-    for size in (1 << 10, 1 << 20, 1 << 21, 1 << 22, 1 << 23, 1 << 24, 1 << 28):
-        for v in pkg.VARIANTS.values():
-            for flags in (0, capi.F_INPUTS_STABLE, capi.F_COLD, capi.F_COLD | capi.F_INPUTS_STABLE):
-                t = pkg.resolve(v, size, flags)           # the geometry of that size class and hint, run on our n
-                out = torch.full((n,), -1.0, dtype=torch.float32, device="cuda")
-                va.add(a, b, out, tune=t)
-                assert_bits_equal(out, want, str(t.as_dict()))
-    for t in (capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=2, st_hint=1, scheduler=1),
-              capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=4, st_hint=1, scheduler=1, early_loads=1)):
+    # the geometry of each size class and hint, run on our n
+    for t in [t for _, t in production_tunes()] + list(k1d_tunes()):
         out = torch.full((n,), -1.0, dtype=torch.float32, device="cuda")
         va.add(a, b, out, tune=t)
+        assert geometry(t, n)[0] == capi.OK, t.as_dict()
         assert_bits_equal(out, want, str(t.as_dict()))
     exotic = capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=8, ld_hint=2, st_hint=2)
     with pytest.raises(pkg.B200VAError) as e:
         va.add(a, b, tune=exotic)
     assert e.value.code == capi.ERR_VARIANT
+    assert geometry(exotic, n)[0] == capi.ERR_VARIANT
     assert_bits_equal(va.add(a, b, tune=exotic, full_matrix=True), want, "tune library")
+    assert geometry(exotic, n, capi.tune_lib())[0] == capi.OK
+
+
+def _profiled_kernel_name(name: str) -> str:
+    """A kernel name as the profiler prints it, in Tune.kernel_name()'s form: no namespace, parameter list, casts
+    or spaces, and bools as 0/1."""
+    name = re.sub(r"\((?:int|bool|unsigned int)\)", "", name).replace("true", "1").replace("false", "0")
+    return re.match(r"(?:void )?(?:b200va::)?(\w+(?:<[^>]*>)?)", name).group(1).replace(" ", "")
+
+
+def test_launched_kernel_has_the_geometry_and_name_the_library_reports(tmp_path):
+    """Every tune the production library resolves, and its K1d tunes, launched once under the profiler on
+    256-byte-aligned buffers of the n it was resolved for: the kernel in the trace has b200va_geometry's grid and
+    block, and Tune.kernel_name() is its name."""
+    cases = {}
+    for size, t in production_tunes() + [(size, t) for size in PRODUCTION_SIZES for t in k1d_tunes()]:
+        cases.setdefault((size, tuple(t.as_dict().values())), t)
+    nmax = max(PRODUCTION_SIZES)
+    a, b, c = (torch.empty(nmax, dtype=torch.float32, device="cuda") for _ in range(3))
+    va.fill_ctr(a, 0x0A)
+    va.fill_ctr(b, 0x0B)
+    assert all(x.data_ptr() % 256 == 0 for x in (a, b, c))
+    torch.cuda.synchronize()
+    want = []
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for (n, _), t in cases.items():
+            rc, grid, block = geometry(t, n)
+            assert rc == capi.OK, t.as_dict()
+            va.add(a[:n], b[:n], c[:n], tune=t)
+            want.append((t.kernel_name(), grid, block, n))
+        torch.cuda.synchronize()
+    trace = tmp_path / "trace.json"
+    prof.export_chrome_trace(str(trace))
+    events = sorted((e for e in json.loads(trace.read_text())["traceEvents"] if e.get("cat") == "kernel"),
+                    key=lambda e: e["ts"])
+    got = [(_profiled_kernel_name(e["name"]), e["args"]["grid"][0], e["args"]["block"][0]) for e in events]
+    assert len(got) == len(want)
+    for g, w in zip(got, want):
+        assert g == w[:3], (g, w)
 
 
 def test_early_loads_chain_of_launches_is_bit_exact():
