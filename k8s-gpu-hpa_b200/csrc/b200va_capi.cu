@@ -785,11 +785,15 @@ int launch_stream_typed(const void* dA, const void* dB, void* dC, size_t n, doub
     fn_t fn = nullptr;
 #ifdef B200VA_TUNE_MATRIX
     if (unroll == 4) fn = skip_l1_stores ? stream_vec<DT, OP, 4, LD_PLAIN, ST_NA> : stream_vec<DT, OP, 4, LD_PLAIN, ST_PLAIN>;
-#endif
-    if (!fn) {
-        if (skip_l1_stores) fn = unroll == 2 ? stream_vec<DT, OP, 2, LD_PLAIN, ST_NA> : stream_vec<DT, OP, 1, LD_PLAIN, ST_NA>;
-        else fn = unroll == 2 ? stream_vec<DT, OP, 2, LD_PLAIN, ST_PLAIN> : stream_vec<DT, OP, 1, LD_PLAIN, ST_PLAIN>;
+    else if (skip_l1_stores) fn = unroll == 2 ? stream_vec<DT, OP, 2, LD_PLAIN, ST_NA> : stream_vec<DT, OP, 1, LD_PLAIN, ST_NA>;
+#else
+    // the production library carries only the ST_NA form the HBM class above picks
+    if (skip_l1_stores) {
+        if constexpr (binary) fn = stream_vec<DT, OP, 1, LD_PLAIN, ST_NA>;
+        else fn = stream_vec<DT, OP, 2, LD_PLAIN, ST_NA>;
     }
+#endif
+    if (!fn) fn = unroll == 2 ? stream_vec<DT, OP, 2, LD_PLAIN, ST_PLAIN> : stream_vec<DT, OP, 1, LD_PLAIN, ST_PLAIN>;
     return launch_kernel(fn, static_cast<unsigned>(grid), threads, 0, st, pdl_enabled(), dA, dB, dC, n, head, nvec, ntiles, s, prefetch_first);
 }
 
