@@ -275,6 +275,41 @@ int b200va_device_numa_node_of(int device);
 int b200va_stream(int op, int dtype, const void *dA, const void *dB, void *dC, size_t n,
                   double scalar, void *stream);
 
+/* ---- reproducible dot product (row f4) --------------------------------------------------
+ * *d_out = sum_i a_i b_i as a binary64 value in device memory, written asynchronously on `stream`
+ * (not rounded to the storage type; dtype is a B200VA_DT_* code).  Every operand is widened
+ * exactly to f64 (f16/bf16 as the stream ops widen them, no FTZ: f32 and f16 subnormals stay).
+ * The result is a function of the values and n only, defined by three rules:
+ *   1. Lane chain: the elements i of chunk k with the same i mod LANES form one lane, which
+ *      accumulates them in increasing index order: acc = +0.0; acc = fma(a_i, b_i, acc) in binary64
+ *      RNE.  For f32/f16/bf16 the product is exact in f64, so this is acc + a_i*b_i rounded once;
+ *      for f64 it is a true fma.
+ *   2. Chunk value: the LANES lane values summed as a pairwise tree over aligned dyadic blocks (the
+ *      value of an aligned block of 2^l entries is the sum of its two halves).  A lane with no
+ *      elements, in the last chunk, is +0.0.
+ *   3. Total: the ceil(n / CHUNK) chunk values summed with the same aligned dyadic tree; where a
+ *      block's upper half is empty, its value is its lower half.  For n = 0 the result is +0.0.
+ * Consequences:
+ *   - The result is never -0.0: the chain starts at +0 and RNE never makes -0 from a sum that is not
+ *     (-0) + (-0).  So "empty lane = +0.0" and "empty lane = absent" give the same bits.
+ *   - The aligned dyadic tree decomposes: any aligned block can be reduced by a different CTA or
+ *     launch and combined later, so how chunks and lanes map onto the GPU does not change the bits.
+ *   - The result is the same at every element offset and any relative alignment of A and B.
+ * Arguments: dA == dB is legal (a sum of squares).  d_workspace is device scratch of at least
+ * b200va_dot_workspace_bytes(n) bytes (NULL allowed when that is 0); only those bytes are written.
+ * B200VA_ERR_VARIANT: bad dtype.  B200VA_ERR_INVALID: NULL d_out, NULL dA/dB/d_workspace with n > 0,
+ * workspace_bytes too small, n > 2^40.  B200VA_ERR_ALIGN: dA/dB not aligned to the element size,
+ * d_out/d_workspace not 8-byte aligned.  B200VA_ERR_OVERLAP: d_out or the workspace overlapping A, B
+ * or each other.  The call never allocates, synchronises or memsets, and is capturable in a CUDA graph:
+ * it is two or more kernel launches on `stream` (a pass over the chunks, then the tree over their
+ * values), the second and later ones behind a programmatic dependency on the one before. */
+#define B200VA_DOT_LANES 2048          /* elements i of a chunk with the same i mod LANES form one lane   */
+#define B200VA_DOT_CHUNK 65536         /* chunk k = indices [k*CHUNK, min(n, (k+1)*CHUNK))                */
+/* Device scratch b200va_dot needs for n elements: 8 * ceil(n / B200VA_DOT_CHUNK) bytes (0 for n = 0). */
+size_t b200va_dot_workspace_bytes(size_t n);
+int b200va_dot(int dtype, const void *dA, const void *dB, size_t n, double *d_out,
+               void *d_workspace, size_t workspace_bytes, void *stream);
+
 /* ---- ceiling probes (measurement aids; not part of the reference's surface) -------------
  * The production launch geometry with one side of the add's traffic removed, so a harness can
  * measure on the spot what the HBM gives each kind of stream (bench.py reports the add as a

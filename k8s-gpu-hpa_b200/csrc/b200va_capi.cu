@@ -30,6 +30,7 @@
 #include "../../include/b200va.h"
 #include "b200va_kernels.cuh"
 #include "b200va_stream.cuh"
+#include "b200va_dot.cuh"
 
 using namespace b200va;
 
@@ -809,6 +810,24 @@ int launch_stream_op(int op, const void* dA, const void* dB, void* dC, size_t n,
     return B200VA_ERR_VARIANT;
 }
 
+// Pass 1 of b200va_dot: one CTA per chunk, one f64 partial each into ws.  The vector form when A and
+// B share a 16-byte phase, else the scalar form; the HBM class of launch_stream_typed (>= 2^25 words
+// per operand) prefetches each CTA's first rows into L2 ahead of the programmatic dependency.
+template <int DT>
+int launch_dot_typed(const void* dA, const void* dB, size_t n, double* ws, cudaStream_t st)
+{
+    constexpr size_t ES = dt_traits<DT>::size;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), b = reinterpret_cast<uintptr_t>(dB);
+    const unsigned grid = static_cast<unsigned>((n + DOT_CHUNK - 1) / DOT_CHUNK);
+    const int prefetch_first = n * ES / 4 >= (size_t{1} << 25) ? 1 : 0;
+    if ((a & 15u) != (b & 15u))
+        return launch_kernel(dot_scalar<DT>, grid, DOT_SCALAR_THREADS, 0, st, pdl_enabled(), dA, dB, n, ws, prefetch_first);
+    using F = dot_form<DT>;
+    const size_t head = ((16u - (a & 15u)) & 15u) / ES;
+    return launch_kernel(dot_vec<DT, F::threads, F::rows>, grid, F::threads, 0, st, pdl_enabled(), dA, dB, n, head, ws,
+                         prefetch_first);
+}
+
 }  // namespace
 
 // =============================================================================== ABI
@@ -1138,6 +1157,54 @@ int b200va_stream(int op, int dtype, const void* dA, const void* dB, void* dC, s
         case DT_BF16: return launch_stream_op<DT_BF16>(op, dA, dB, dC, n, scalar, st);
     }
     return B200VA_ERR_VARIANT;
+}
+
+size_t b200va_dot_workspace_bytes(size_t n)
+{
+    return 8 * (n / DOT_CHUNK + (n % DOT_CHUNK != 0));
+}
+
+int b200va_dot(int dtype, const void* dA, const void* dB, size_t n, double* d_out, void* d_workspace,
+               size_t workspace_bytes, void* stream)
+{
+    if (dtype < 0 || dtype >= DT_COUNT) return B200VA_ERR_VARIANT;
+    const b200va_devinfo_t* di = nullptr;
+    RC_TRY(current_dev_info(&di));
+    if (n > (size_t{1} << 40)) return B200VA_ERR_INVALID;
+    const size_t need = b200va_dot_workspace_bytes(n);
+    if (!d_out || (n && (!dA || !dB)) || (need && !d_workspace) || workspace_bytes < need) return B200VA_ERR_INVALID;
+    const size_t es = dtype == DT_F64 ? 8 : dtype == DT_F32 ? 4 : 2;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), b = reinterpret_cast<uintptr_t>(dB),
+                    o = reinterpret_cast<uintptr_t>(d_out), w = reinterpret_cast<uintptr_t>(d_workspace);
+    if (n && ((a | b) & (es - 1)) != 0) return B200VA_ERR_ALIGN;
+    if ((o & 7u) || (need && (w & 7u))) return B200VA_ERR_ALIGN;
+    // what the call writes (d_out, the needed workspace) must not meet what it reads or each other
+    auto meet = [](uintptr_t x, size_t xn, uintptr_t y, size_t yn) { return xn && yn && x < y + yn && y < x + xn; };
+    const size_t bytes = n * es;
+    if (meet(o, 8, a, bytes) || meet(o, 8, b, bytes) || meet(o, 8, w, need) || meet(w, need, a, bytes) ||
+        meet(w, need, b, bytes))
+        return B200VA_ERR_OVERLAP;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    double* ws = static_cast<double*>(d_workspace);
+    if (n) {
+        switch (dtype) {
+            case DT_F32:  RC_TRY(launch_dot_typed<DT_F32>(dA, dB, n, ws, st)); break;
+            case DT_F64:  RC_TRY(launch_dot_typed<DT_F64>(dA, dB, n, ws, st)); break;
+            case DT_F16:  RC_TRY(launch_dot_typed<DT_F16>(dA, dB, n, ws, st)); break;
+            case DT_BF16: RC_TRY(launch_dot_typed<DT_BF16>(dA, dB, n, ws, st)); break;
+        }
+    }
+    // pass 2: aligned blocks of DOT_FINAL_BLOCK partials per CTA, one level per launch, until one CTA
+    // writes *d_out (for n = 0 it sums nothing and writes +0.0)
+    size_t k = need / 8, stride = 1;
+    while (k > static_cast<size_t>(DOT_FINAL_BLOCK)) {
+        const size_t grid = (k + DOT_FINAL_BLOCK - 1) / DOT_FINAL_BLOCK;
+        RC_TRY(launch_kernel(dot_final, static_cast<unsigned>(grid), DOT_FINAL_THREADS, 0, st, pdl_enabled(), ws, k, stride,
+                             static_cast<double*>(nullptr)));
+        k = grid;
+        stride *= DOT_FINAL_BLOCK;
+    }
+    return launch_kernel(dot_final, 1u, DOT_FINAL_THREADS, 0, st, pdl_enabled(), ws, k, stride, d_out);
 }
 
 // ------------------------------------------------------------------ ceiling probes

@@ -135,6 +135,40 @@ def stream(op: str, a, b=None, out=None, *, scalar: float = 0.0, stream=None):
     return out
 
 
+def dot(a, b, *, out=None, workspace=None, stream=None):
+    """The reproducible dot product of two equal-length contiguous CUDA tensors of one of f32/f64/f16/bf16
+    (b200va_dot): a 0-d float64 CUDA tensor, written asynchronously on the current stream.  The bits
+    depend on the values and the length only.  ``out``: a float64 CUDA tensor of at least one element to
+    write the result into (its first element); ``workspace``: a CUDA tensor of at least
+    b200va_dot_workspace_bytes(n) bytes, else one is taken from the torch allocator for this call."""
+    torch = _torch()
+    names = {getattr(torch, v): k for k, v in _TORCH_DT.items()}
+    for name, t in (("a", a), ("b", b)):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype not in names or not t.is_contiguous():
+            raise TypeError(f"{name} must be a contiguous CUDA tensor of float32/float64/float16/bfloat16")
+    if b.dtype != a.dtype or b.numel() != a.numel() or b.device != a.device:
+        raise TypeError("a and b must match in dtype, length and device")
+    n = a.numel()
+    need = lib.b200va_dot_workspace_bytes(n)
+    if out is None:
+        out = torch.empty((), dtype=torch.float64, device=a.device)
+    elif (not isinstance(out, torch.Tensor) or out.dtype != torch.float64 or out.device != a.device
+          or out.numel() < 1 or not out.is_contiguous()):
+        raise TypeError("out must be a contiguous float64 tensor on a's device")
+    if workspace is not None and (not isinstance(workspace, torch.Tensor) or workspace.device != a.device
+                                  or not workspace.is_contiguous()):
+        raise TypeError("workspace must be a contiguous tensor on a's device")
+    with torch.cuda.device(a.device):
+        if workspace is None:
+            # allocated on the stream the call runs on, so the allocator reuses it only after that stream's work
+            with torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream()):
+                workspace = torch.empty(max(need, 8), dtype=torch.uint8, device=a.device)
+        check(lib.b200va_dot(capi.DTYPES[names[a.dtype]], a.data_ptr(), b.data_ptr(), n, out.data_ptr(),
+                             workspace.data_ptr(), workspace.numel() * workspace.element_size(), _stream_ptr(stream)),
+              "b200va_dot")
+    return out
+
+
 def probe(kind: str, a, b, c, *, stream=None):
     """Ceiling probe (b200va_probe_f32): 'read2' loads a and b, 'fill' stores c, 'copy' c = a.  c is clobbered."""
     torch = _torch()
