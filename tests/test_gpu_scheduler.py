@@ -3,7 +3,7 @@ written exactly once, also when a ticket counter is used again.
 
 A dynamically scheduled launch claims tiles from a two-word counter that must be zero when it starts; its last CTA
 zeroes the counter again.  Direct launches take their counter from the device's ring of 4096 slots, a loop handle's
-graph from the handle (csrc/b200va_capi.cu: sched_slot, b200va_loop).  A counter that is not zero makes a launch
+graph from the handle (csrc/b200va_add.cu: sched_slot, b200va_loop).  A counter that is not zero makes a launch
 skip tiles and report nothing, so every launch here writes into an output poisoned beforehand with a finite pattern
 and is verified afterwards: the device recompute, the oracle's digest, and the oracle element by element on windows
 at the head, the middle and the ragged tail, plus guard elements on both sides that must keep the poison.  Most
