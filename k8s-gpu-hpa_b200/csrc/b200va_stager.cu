@@ -117,27 +117,36 @@ static CopyPool* make_copy_pool()
 
 struct HostRange { uintptr_t lo, hi; };     // [lo, hi) page-locked by this stager (mode 4)
 
+namespace {    // internal linkage: std::vector<Slot>'s code stays out of the libraries' symbol tables
+// One of the `depth` device slots a chunk rotates through.
+struct Slot {
+    float* d = nullptr;                  // A, B and C of one chunk, `chunk` floats each (in d_buf)
+    cudaStream_t stream = nullptr;       // mode 0: the chunk's copies and add
+    cudaEvent_t in = nullptr, sum = nullptr, out = nullptr;   // A and B arrived, C computed, C copied out
+    size_t off = 0, m = 0;               // the chunk it holds: where it sits in the caller's arrays, its length
+};
+}  // namespace
+
 struct b200va_stager {
     int device = 0;
     size_t chunk = 0;
-    int depth = 0;
-    float* d_buf = nullptr;            // depth * 3 * chunk floats
+    float* d_buf = nullptr;              // the slots: depth * 3 * chunk floats
+    std::vector<Slot> slots;
     cudaStream_t main = nullptr;
-    cudaStream_t* slot = nullptr;
-    cudaEvent_t* slot_done = nullptr;
-    cudaEvent_t ev_start = nullptr, ev_stop = nullptr;
-    // "lanes" pipeline (mode 2): one stream per direction + one for the kernel, events per slot
+    // modes 2, 3 and 4: one stream for the H2D copies, one for the adds, one for the D2H copies
     cudaStream_t lane_h2d = nullptr, lane_k = nullptr, lane_d2h = nullptr;
-    cudaEvent_t *ev_in = nullptr, *ev_sum = nullptr, *ev_out = nullptr;
-    // pageable path (mode 3): pinned bounce chunks (depth * 3 * bounce_chunk floats) + copy threads, made on first use
+    cudaEvent_t ev_start = nullptr, ev_stop = nullptr;
+    // pageable path (mode 3): pinned bounce slots (depth * 3 * bounce_chunk(s) floats) + copy threads, made on first use
     float* bounce = nullptr;
-    size_t bounce_chunk = 0;
     CopyPool* pool = nullptr;
     // register-once path (mode 4): host ranges this stager page-locked
-    std::vector<HostRange>* regs = nullptr;
+    std::vector<HostRange> regs;
     float last_ms = 0.f;
     int last_mode = -1;
 };
+
+// Mode 3's chunk length, and the length of each array of a bounce slot: 32 MiB at most.
+static size_t bounce_chunk(const b200va_stager* s) { return std::min(s->chunk, size_t{1} << 23); }
 
 // NUMA node a CUDA device hangs off (sysfs), or -1.  B200VA_NUMA_NODE overrides.
 static int device_numa_node_of(int dev)
@@ -245,10 +254,9 @@ int b200va_host_free(void* p)
 
 static void stager_release_host(b200va_stager* s)
 {
-    if (!s->regs) return;
-    for (const HostRange& r : *s->regs)
+    for (const HostRange& r : s->regs)
         if (cudaHostUnregister(reinterpret_cast<void*>(r.lo)) != cudaSuccess) cudaGetLastError();
-    s->regs->clear();
+    s->regs.clear();
 }
 
 int b200va_stager_release_host(b200va_stager_t* s)
@@ -264,30 +272,44 @@ int b200va_stager_destroy(b200va_stager_t* s)
     if (!s) return B200VA_OK;
     DeviceGuard g(s->device);
     stager_release_host(s);
-    delete s->regs;
-    if (s->slot) {
-        for (int i = 0; i < s->depth; ++i) {
-            if (s->slot[i]) cudaStreamDestroy(s->slot[i]);
-            if (s->slot_done && s->slot_done[i]) cudaEventDestroy(s->slot_done[i]);
-        }
+    for (const Slot& sl : s->slots) {
+        if (sl.stream) cudaStreamDestroy(sl.stream);
+        for (cudaEvent_t ev : {sl.in, sl.sum, sl.out})
+            if (ev) cudaEventDestroy(ev);
     }
-    for (cudaStream_t st : {s->lane_h2d, s->lane_k, s->lane_d2h})
+    for (cudaStream_t st : {s->main, s->lane_h2d, s->lane_k, s->lane_d2h})
         if (st) cudaStreamDestroy(st);
-    for (cudaEvent_t* arr : {s->ev_in, s->ev_sum, s->ev_out}) {
-        if (!arr) continue;
-        for (int i = 0; i < s->depth; ++i)
-            if (arr[i]) cudaEventDestroy(arr[i]);
-        delete[] arr;
-    }
-    if (s->main) cudaStreamDestroy(s->main);
-    if (s->ev_start) cudaEventDestroy(s->ev_start);
-    if (s->ev_stop) cudaEventDestroy(s->ev_stop);
+    for (cudaEvent_t ev : {s->ev_start, s->ev_stop})
+        if (ev) cudaEventDestroy(ev);
     if (s->d_buf) cudaFree(s->d_buf);
     if (s->bounce) cudaFreeHost(s->bounce);
     delete s->pool;
-    delete[] s->slot;
-    delete[] s->slot_done;
     delete s;
+    return B200VA_OK;
+}
+
+// Makes everything a stager owns; on failure the caller destroys what was made.
+static int stager_make(b200va_stager* s, int device, size_t chunk, int depth)
+{
+    s->device = device;
+    s->chunk = chunk;
+    try {
+        s->slots.resize(static_cast<size_t>(depth));
+    } catch (const std::bad_alloc&) {
+        return B200VA_ERR_NOMEM;
+    }
+    CU_TRY(cudaMalloc(&s->d_buf, s->slots.size() * 3 * s->chunk * sizeof(float)));
+    for (cudaStream_t* st : {&s->main, &s->lane_h2d, &s->lane_k, &s->lane_d2h})
+        CU_TRY(cudaStreamCreateWithFlags(st, cudaStreamNonBlocking));
+    CU_TRY(cudaEventCreate(&s->ev_start));
+    CU_TRY(cudaEventCreate(&s->ev_stop));
+    for (size_t i = 0; i < s->slots.size(); ++i) {
+        Slot& sl = s->slots[i];
+        sl.d = s->d_buf + i * 3 * s->chunk;
+        CU_TRY(cudaStreamCreateWithFlags(&sl.stream, cudaStreamNonBlocking));
+        for (cudaEvent_t* ev : {&sl.in, &sl.sum, &sl.out})
+            CU_TRY(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
+    }
     return B200VA_OK;
 }
 
@@ -303,34 +325,8 @@ int b200va_stager_create(b200va_stager_t** out, int device, size_t chunk_elems, 
     DeviceGuard guard(device);
     CU_TRY(guard.err);
     b200va_stager* s = new (std::nothrow) b200va_stager;
-    if (!s) return B200VA_ERR_NOMEM;
-    s->device = device;
-    s->chunk = chunk_elems;
-    s->depth = depth;
-    s->slot = new (std::nothrow) cudaStream_t[depth]();
-    s->slot_done = new (std::nothrow) cudaEvent_t[depth]();
-    s->regs = new (std::nothrow) std::vector<HostRange>();
-    if (!s->slot || !s->slot_done || !s->regs) { b200va_stager_destroy(s); return B200VA_ERR_NOMEM; }
-    cudaError_t e = cudaMalloc(&s->d_buf, static_cast<size_t>(depth) * 3 * chunk_elems * sizeof(float));
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s->main, cudaStreamNonBlocking);
-    for (int i = 0; i < depth && e == cudaSuccess; ++i) {
-        e = cudaStreamCreateWithFlags(&s->slot[i], cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->slot_done[i], cudaEventDisableTiming);
-    }
-    if (e == cudaSuccess) e = cudaEventCreate(&s->ev_start);
-    if (e == cudaSuccess) e = cudaEventCreate(&s->ev_stop);
-    s->ev_in = new (std::nothrow) cudaEvent_t[depth]();
-    s->ev_sum = new (std::nothrow) cudaEvent_t[depth]();
-    s->ev_out = new (std::nothrow) cudaEvent_t[depth]();
-    if (!s->ev_in || !s->ev_sum || !s->ev_out) { b200va_stager_destroy(s); return B200VA_ERR_NOMEM; }
-    for (cudaStream_t* st : {&s->lane_h2d, &s->lane_k, &s->lane_d2h})
-        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(st, cudaStreamNonBlocking);
-    for (int i = 0; i < depth && e == cudaSuccess; ++i) {
-        e = cudaEventCreateWithFlags(&s->ev_in[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev_sum[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev_out[i], cudaEventDisableTiming);
-    }
-    if (e != cudaSuccess) { b200va_stager_destroy(s); return cuda_err(e); }
+    const int rc = s ? stager_make(s, device, chunk_elems, depth) : B200VA_ERR_NOMEM;
+    if (rc != B200VA_OK) { b200va_stager_destroy(s); return rc; }
     *out = s;
     return B200VA_OK;
 }
@@ -352,33 +348,8 @@ static int stage_zero_copy(b200va_stager* s, const float* hA, const float* hB, f
     return launch(dA, dB, dC, n, t, s->main, pdl_enabled());
 }
 
-static int stage_slots(b200va_stager* s, const float* hA, const float* hB, float* hC, size_t n, int variant)
-{
-    const size_t nchunks = (n + s->chunk - 1) / s->chunk;
-    for (int i = 0; i < s->depth; ++i) CU_TRY(cudaStreamWaitEvent(s->slot[i], s->ev_start, 0));
-    b200va_tune_t t;
-    for (size_t k = 0; k < nchunks; ++k) {
-        const int i = static_cast<int>(k % static_cast<size_t>(s->depth));
-        const size_t off = k * s->chunk;
-        const size_t m = (n - off < s->chunk) ? n - off : s->chunk;
-        float* dA = s->d_buf + static_cast<size_t>(i) * 3 * s->chunk;
-        float* dB = dA + s->chunk;
-        float* dC = dB + s->chunk;
-        CU_TRY(cudaMemcpyAsync(dA, hA + off, m * sizeof(float), cudaMemcpyHostToDevice, s->slot[i]));
-        CU_TRY(cudaMemcpyAsync(dB, hB + off, m * sizeof(float), cudaMemcpyHostToDevice, s->slot[i]));
-        default_tune(variant, m, &t, B200VA_F_COLD);      // a chunk fresh off the copy engine is never in L2
-        RC_TRY(launch(dA, dB, dC, m, t, s->slot[i], pdl_enabled()));
-        CU_TRY(cudaMemcpyAsync(hC + off, dC, m * sizeof(float), cudaMemcpyDeviceToHost, s->slot[i]));
-    }
-    for (int i = 0; i < s->depth; ++i) {
-        CU_TRY(cudaEventRecord(s->slot_done[i], s->slot[i]));
-        CU_TRY(cudaStreamWaitEvent(s->main, s->slot_done[i], 0));
-    }
-    return B200VA_OK;
-}
-
 // Fault injection for the error-path test (tests/test_gpu_host_path.py): with
-// B200VA_TEST_FAIL_CHUNK=k in the environment the lanes pipeline fails ONCE per process, right
+// B200VA_TEST_FAIL_CHUNK=k in the environment the chunk loop fails ONCE per process, right
 // after it has queued chunk k's H2D copies -- i.e. with DMA in flight on the caller's arrays.
 static bool inject_fault_at_chunk(size_t k)
 {
@@ -387,106 +358,82 @@ static bool inject_fault_at_chunk(size_t k)
     return at >= 0 && static_cast<long>(k) == at && !fired.exchange(true);
 }
 
-static int stage_lanes(b200va_stager* s, const float* hA, const float* hB, float* hC, size_t n, int variant)
+// The length of the next chunk when `left` elements are still to be staged.
+static size_t chunk_len(const b200va_stager* s, int mode, size_t left)
 {
-    // lanes: every H2D copy queues on one stream, every add on a second, every D2H on a
-    // third; slot reuse and data flow are event edges.  The H2D queue -- the bottleneck
-    // direction -- never waits behind a kernel or a D2H of another chunk.
-    for (cudaStream_t st : {s->lane_h2d, s->lane_k, s->lane_d2h}) CU_TRY(cudaStreamWaitEvent(st, s->ev_start, 0));
-    b200va_tune_t t;
-    // Full-size chunks, then a tapered tail (1/2, 1/4, ... down to ~1 Mi elements): what is left
+    if (mode == B200VA_STAGE_BOUNCE) return std::min(bounce_chunk(s), left);
+    if (mode == B200VA_STAGE_SLOTS || left > s->chunk || s->slots.size() == 1) return std::min(s->chunk, left);
+    // Modes 2 and 4: full-size chunks, then a tapered tail (1/2, 1/4, ... down to ~1 Mi elements): what is left
     // after the last H2D byte has arrived is one small add and one small D2H, not a full chunk.
-    const size_t taper_min = size_t{1} << 20;
-    size_t off = 0;
-    for (size_t k = 0; off < n; ++k) {
-        const size_t left = n - off;
-        size_t m = s->chunk;
-        if (left <= s->chunk && s->depth > 1) {
-            m = left / 2;
-            m = (m + 63) & ~size_t{63};                      // chunk starts stay 256-byte aligned
-            if (m < taper_min || m >= left) m = left;
-        }
-        if (m > left) m = left;
-        const int i = static_cast<int>(k % static_cast<size_t>(s->depth));
-        float* dA = s->d_buf + static_cast<size_t>(i) * 3 * s->chunk;
-        float* dB = dA + s->chunk;
-        float* dC = dB + s->chunk;
-        if (k >= static_cast<size_t>(s->depth)) CU_TRY(cudaStreamWaitEvent(s->lane_h2d, s->ev_out[i], 0));  // slot drained
-        CU_TRY(cudaMemcpyAsync(dA, hA + off, m * sizeof(float), cudaMemcpyHostToDevice, s->lane_h2d));
-        CU_TRY(cudaMemcpyAsync(dB, hB + off, m * sizeof(float), cudaMemcpyHostToDevice, s->lane_h2d));
-        CU_TRY(cudaEventRecord(s->ev_in[i], s->lane_h2d));
-        if (inject_fault_at_chunk(k)) return B200VA_ERR_INVALID;   // test hook: fail with copies in flight
-        CU_TRY(cudaStreamWaitEvent(s->lane_k, s->ev_in[i], 0));
-        default_tune(variant, m, &t, B200VA_F_COLD);      // a chunk fresh off the copy engine is never in L2
-        RC_TRY(launch(dA, dB, dC, m, t, s->lane_k, pdl_enabled()));
-        CU_TRY(cudaEventRecord(s->ev_sum[i], s->lane_k));
-        CU_TRY(cudaStreamWaitEvent(s->lane_d2h, s->ev_sum[i], 0));
-        CU_TRY(cudaMemcpyAsync(hC + off, dC, m * sizeof(float), cudaMemcpyDeviceToHost, s->lane_d2h));
-        CU_TRY(cudaEventRecord(s->ev_out[i], s->lane_d2h));
-        off += m;
-    }
-    CU_TRY(cudaEventRecord(s->slot_done[0], s->lane_d2h));   // the D2H lane finishes last
-    CU_TRY(cudaStreamWaitEvent(s->main, s->slot_done[0], 0));
-    return B200VA_OK;
+    const size_t m = (left / 2 + 63) & ~size_t{63};          // chunk starts stay 256-byte aligned
+    return m < (size_t{1} << 20) || m >= left ? left : m;
 }
 
-static int stage_bounce(b200va_stager* s, const float* hA, const float* hB, float* hC, size_t n, int variant)
+// Modes 0, 2, 3 and 4: the vector in chunks that rotate through the slots; each chunk is two H2D copies, the add
+// and a D2H copy.  Mode 0 queues a chunk's work on its slot's stream.  The other modes queue every H2D copy on one
+// lane, every add on a second and every D2H copy on a third, with data flow and slot reuse as event edges, so the
+// H2D lane -- the bottleneck direction -- never waits behind another chunk's add or D2H.
+// Mode 3 takes pageable arrays (plain malloc, what one ./vectorAdd process has), which the driver would stage on
+// one thread at ~10 GB/s: a pool of host threads copies each chunk into a pinned bounce slot before its H2D, and
+// out of it depth - 1 chunks later, while the copy engines and the add work on the chunks in between.
+static int stage_chunks(b200va_stager* s, const float* hA, const float* hB, float* hC, size_t n, int variant, int mode)
 {
-    // Pageable host arrays (plain malloc, what one ./vectorAdd process has): a cudaMemcpy from
-    // pageable memory is staged by the driver on one thread at ~10 GB/s.  Here a pool of host
-    // threads copies chunk k+1 into pinned bounce buffers and chunk k-2 out of them while the
-    // copy engines and the add work on the chunks in between (lanes as in mode 2).
-    const size_t bc = std::min(s->chunk, size_t{1} << 23);          // 32 MiB bounce chunks
-    if (!s->pool) {
-        s->pool = make_copy_pool();
-        if (!s->pool) return B200VA_ERR_NOMEM;
-    }
-    if (!s->bounce || s->bounce_chunk != bc) {
-        if (s->bounce) { cudaFreeHost(s->bounce); s->bounce = nullptr; }
+    const bool lanes = mode != B200VA_STAGE_SLOTS, bounce = mode == B200VA_STAGE_BOUNCE;
+    const size_t depth = s->slots.size(), bc = bounce_chunk(s);
+    if (bounce && !s->pool && !(s->pool = make_copy_pool())) return B200VA_ERR_NOMEM;
+    if (bounce && !s->bounce) {
         void* p = nullptr;
-        RC_TRY(b200va_host_alloc(&p, static_cast<size_t>(s->depth) * 3 * bc * sizeof(float)));
+        RC_TRY(b200va_host_alloc(&p, depth * 3 * bc * sizeof(float)));
         s->bounce = static_cast<float*>(p);
-        s->bounce_chunk = bc;
     }
-    for (cudaStream_t st : {s->lane_h2d, s->lane_k, s->lane_d2h}) CU_TRY(cudaStreamWaitEvent(st, s->ev_start, 0));
-    const size_t nchunks = (n + bc - 1) / bc;
-    const size_t depth = static_cast<size_t>(s->depth);
+    // mode 3: chunk j's result leaves its bounce slot for the caller's C once its D2H has landed
+    auto retire = [&](size_t j) -> int {
+        const Slot& sl = s->slots[j % depth];
+        CU_TRY(cudaEventSynchronize(sl.out));
+        s->pool->copy(hC + sl.off, s->bounce + (j % depth) * 3 * bc + 2 * bc, sl.m * sizeof(float));
+        return B200VA_OK;
+    };
     b200va_tune_t t;
-    auto span = [&](size_t k, size_t* off, size_t* m) { *off = k * bc; *m = std::min(bc, n - *off); };
-    for (size_t k = 0; k < nchunks + depth - 1 || k < nchunks; ++k) {
-        if (k < nchunks) {
-            size_t off, m;
-            span(k, &off, &m);
-            const size_t i = k % depth;
-            float* pA = s->bounce + i * 3 * bc;
-            float* dA = s->d_buf + i * 3 * s->chunk;
-            // slot i was drained (copied out) at iteration k-1 below, or never used
-            s->pool->copy(pA, hA + off, m * sizeof(float));
-            s->pool->copy(pA + bc, hB + off, m * sizeof(float));
-            CU_TRY(cudaMemcpyAsync(dA, pA, m * sizeof(float), cudaMemcpyHostToDevice, s->lane_h2d));
-            CU_TRY(cudaMemcpyAsync(dA + s->chunk, pA + bc, m * sizeof(float), cudaMemcpyHostToDevice, s->lane_h2d));
-            CU_TRY(cudaEventRecord(s->ev_in[i], s->lane_h2d));
-            CU_TRY(cudaStreamWaitEvent(s->lane_k, s->ev_in[i], 0));
-            default_tune(variant, m, &t, B200VA_F_COLD);
-            RC_TRY(launch(dA, dA + s->chunk, dA + 2 * s->chunk, m, t, s->lane_k, pdl_enabled()));
-            CU_TRY(cudaEventRecord(s->ev_sum[i], s->lane_k));
-            CU_TRY(cudaStreamWaitEvent(s->lane_d2h, s->ev_sum[i], 0));
-            CU_TRY(cudaMemcpyAsync(pA + 2 * bc, dA + 2 * s->chunk, m * sizeof(float), cudaMemcpyDeviceToHost, s->lane_d2h));
-            CU_TRY(cudaEventRecord(s->ev_out[i], s->lane_d2h));
+    size_t k = 0;
+    for (size_t off = 0; off < n; ++k) {
+        const size_t i = k % depth, m = chunk_len(s, mode, n - off);
+        Slot& sl = s->slots[i];
+        cudaStream_t h2d = lanes ? s->lane_h2d : sl.stream, add = lanes ? s->lane_k : sl.stream,
+                     d2h = lanes ? s->lane_d2h : sl.stream;
+        // A slot's first chunk in this call follows the call's start, a later one the previous chunk's D2H out of
+        // the slot (in mode 0 that is stream order; in mode 3 the host has already waited for it, in retire).
+        CU_TRY(cudaStreamWaitEvent(h2d, k < depth ? s->ev_start : sl.out, 0));
+        sl.off = off;
+        sl.m = m;
+        const float *srcA = hA + off, *srcB = hB + off;
+        float* dstC = hC + off;
+        if (bounce) {                                        // the bounce slot was retired at iteration k-1, or never used
+            float* p = s->bounce + i * 3 * bc;
+            s->pool->copy(p, srcA, m * sizeof(float));
+            s->pool->copy(p + bc, srcB, m * sizeof(float));
+            srcA = p;
+            srcB = p + bc;
+            dstC = p + 2 * bc;
         }
-        if (k + 1 >= depth) {                                       // retire chunk j = k - (depth - 1)
-            const size_t j = k + 1 - depth;
-            if (j < nchunks) {
-                size_t off, m;
-                span(j, &off, &m);
-                const size_t i = j % depth;
-                CU_TRY(cudaEventSynchronize(s->ev_out[i]));
-                s->pool->copy(hC + off, s->bounce + i * 3 * bc + 2 * bc, m * sizeof(float));
-            }
-        }
+        float *dA = sl.d, *dB = dA + s->chunk, *dC = dB + s->chunk;
+        CU_TRY(cudaMemcpyAsync(dA, srcA, m * sizeof(float), cudaMemcpyHostToDevice, h2d));
+        CU_TRY(cudaMemcpyAsync(dB, srcB, m * sizeof(float), cudaMemcpyHostToDevice, h2d));
+        CU_TRY(cudaEventRecord(sl.in, h2d));
+        if (inject_fault_at_chunk(k)) return B200VA_ERR_INVALID;   // test hook: fail with copies in flight
+        CU_TRY(cudaStreamWaitEvent(add, sl.in, 0));
+        default_tune(variant, m, &t, B200VA_F_COLD);      // a chunk fresh off the copy engine is never in L2
+        RC_TRY(launch(dA, dB, dC, m, t, add, pdl_enabled()));
+        CU_TRY(cudaEventRecord(sl.sum, add));
+        CU_TRY(cudaStreamWaitEvent(d2h, sl.sum, 0));
+        CU_TRY(cudaMemcpyAsync(dstC, dC, m * sizeof(float), cudaMemcpyDeviceToHost, d2h));
+        CU_TRY(cudaEventRecord(sl.out, d2h));
+        if (bounce && k + 1 >= depth) RC_TRY(retire(k + 1 - depth));
+        off += m;
     }
-    CU_TRY(cudaEventRecord(s->slot_done[0], s->lane_d2h));
-    CU_TRY(cudaStreamWaitEvent(s->main, s->slot_done[0], 0));
+    if (bounce)                                              // the last depth - 1 chunks are still in the ring
+        for (size_t j = k + 1 > depth ? k + 1 - depth : 0; j < k; ++j) RC_TRY(retire(j));
+    // the call ends after every used slot's last D2H (on the D2H lane, the last one follows all the others)
+    for (size_t i = 0; i < std::min(k, depth); ++i) CU_TRY(cudaStreamWaitEvent(s->main, s->slots[i].out, 0));
     return B200VA_OK;
 }
 
@@ -505,15 +452,15 @@ static bool ensure_registered(b200va_stager* s, const void* p, size_t bytes)
 {
     if (bytes == 0) return true;
     const uintptr_t lo = reinterpret_cast<uintptr_t>(p), hi = lo + bytes;
-    for (const HostRange& r : *s->regs)
+    for (const HostRange& r : s->regs)
         if (r.lo <= lo && hi <= r.hi) return true;                  // cached
     if (host_is_pinned(p) && host_is_pinned(reinterpret_cast<const void*>(hi - 1))) return true;
     // a cached range that overlaps without containing the new one (the caller's buffer moved or grew): drop it
-    for (size_t i = 0; i < s->regs->size();) {
-        const HostRange r = (*s->regs)[i];
+    for (size_t i = 0; i < s->regs.size();) {
+        const HostRange r = s->regs[i];
         if (r.lo < hi && lo < r.hi) {
             if (cudaHostUnregister(reinterpret_cast<void*>(r.lo)) != cudaSuccess) cudaGetLastError();
-            s->regs->erase(s->regs->begin() + static_cast<long>(i));
+            s->regs.erase(s->regs.begin() + static_cast<long>(i));
         } else {
             ++i;
         }
@@ -521,7 +468,7 @@ static bool ensure_registered(b200va_stager* s, const void* p, size_t bytes)
     const cudaError_t e = cudaHostRegister(const_cast<void*>(p), bytes, cudaHostRegisterPortable);
     if (e != cudaSuccess) { cudaGetLastError(); return false; }
     try {
-        s->regs->push_back(HostRange{lo, hi});
+        s->regs.push_back(HostRange{lo, hi});
     } catch (...) {
         cudaHostUnregister(const_cast<void*>(p));
         return false;
@@ -533,10 +480,8 @@ static void stager_drain(b200va_stager* s)
 {
     // after a failure in the middle of a pipeline: nothing may still be reading or writing the
     // caller's arrays (or the bounce ring) when the error code is returned
-    for (int i = 0; i < s->depth; ++i)
-        if (s->slot && s->slot[i]) cudaStreamSynchronize(s->slot[i]);
-    for (cudaStream_t st : {s->lane_h2d, s->lane_k, s->lane_d2h, s->main})
-        if (st) cudaStreamSynchronize(st);
+    for (const Slot& sl : s->slots) cudaStreamSynchronize(sl.stream);
+    for (cudaStream_t st : {s->lane_h2d, s->lane_k, s->lane_d2h, s->main}) cudaStreamSynchronize(st);
     cudaGetLastError();
 }
 
@@ -560,14 +505,8 @@ int b200va_stager_add_f32(b200va_stager_t* s, const float* hA, const float* hB, 
     }
     s->last_mode = mode;
     CU_TRY(cudaEventRecord(s->ev_start, s->main));
-    int rc = B200VA_OK;
-    switch (mode) {
-        case B200VA_STAGE_ZEROCOPY: rc = stage_zero_copy(s, hA, hB, hC, n, variant); break;
-        case B200VA_STAGE_SLOTS:    rc = stage_slots(s, hA, hB, hC, n, variant); break;
-        case B200VA_STAGE_LANES:
-        case B200VA_STAGE_REGISTER: rc = stage_lanes(s, hA, hB, hC, n, variant); break;
-        case B200VA_STAGE_BOUNCE:   rc = stage_bounce(s, hA, hB, hC, n, variant); break;
-    }
+    int rc = mode == B200VA_STAGE_ZEROCOPY ? stage_zero_copy(s, hA, hB, hC, n, variant)
+                                           : stage_chunks(s, hA, hB, hC, n, variant, mode);
     if (rc == B200VA_OK) rc = cuda_err(cudaEventRecord(s->ev_stop, s->main));
     if (rc == B200VA_OK) rc = cuda_err(cudaStreamSynchronize(s->main));
     if (rc != B200VA_OK) { stager_drain(s); return rc; }

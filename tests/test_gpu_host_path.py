@@ -189,7 +189,7 @@ def test_stager_restores_the_callers_current_device():
         assert y.device.index == before and float(y.sum()) == 2048.0
 
 
-def test_stager_error_in_the_middle_leaves_nothing_in_flight():
+def _fail_in_the_middle(mode: int) -> None:
     """A failure in the middle of the pipeline (injected right after chunk 1's H2D copies were
     queued) returns an error code only after every stream of the stager has drained: the caller
     may overwrite or free its arrays at once, and the stager works on the next call."""
@@ -200,26 +200,28 @@ def test_stager_error_in_the_middle_leaves_nothing_in_flight():
 
     from conftest import ROOT
 
-    code = textwrap.dedent("""
+    code = textwrap.dedent(f"""
         import numpy as np, torch, oracle
         from k8s_gpu_hpa_b200 import capi, vector_add as va
-        n = 6 * (1 << 20) + 11
+        mode, n = {mode}, 6 * (1 << 20) + 11
         ha = torch.from_numpy(oracle.fill_ctr(n, 0x0A)).pin_memory()
         hb = torch.from_numpy(oracle.fill_ctr(n, 0x0B)).pin_memory()
         hc = torch.full((n,), -1.0).pin_memory()
         want = oracle.vadd(ha.numpy(), hb.numpy())
         with va.Stager(0, 1 << 20, 3) as st:
             try:
-                st.add(ha, hb, hc, mode=capi.STAGE_LANES)
+                st.add(ha, hb, hc, mode=mode)
                 raise SystemExit("the injected fault did not surface")
             except capi.B200VAError as e:
                 assert e.code == capi.ERR_INVALID, e
-            # drained: chunk 0 completed (its D2H landed), nothing of chunk 2.. was ever started
+            # drained: nothing of chunk 2.. was ever started, and chunk 0 completed (its D2H landed) -- in mode 3
+            # its result would leave the bounce ring for C only two chunks later
             got = hc.numpy()
-            assert oracle.first_mismatch(got[:1 << 20].copy(), want[:1 << 20].copy()) == -1
+            if mode != capi.STAGE_BOUNCE:
+                assert oracle.first_mismatch(got[:1 << 20].copy(), want[:1 << 20].copy()) == -1
             assert (got[2 << 20:] == -1.0).all()
             ha.zero_(); ha.copy_(torch.from_numpy(oracle.fill_ctr(n, 0x0A)))   # scribbling over A right away is safe
-            st.add(ha, hb, hc, mode=capi.STAGE_LANES)                           # the hook fires once: this call is clean
+            st.add(ha, hb, hc, mode=mode)                                       # the hook fires once: this call is clean
             assert oracle.first_mismatch(hc.numpy(), want) == -1
         x = torch.ones(16, device="cuda")
         assert float(va.add(x, x).sum()) == 32.0                                 # no latched CUDA error either
@@ -228,6 +230,15 @@ def test_stager_error_in_the_middle_leaves_nothing_in_flight():
     p = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600, cwd=ROOT,
                        env=dict(os.environ, B200VA_TEST_FAIL_CHUNK="1", PYTHONPATH=ROOT))
     assert p.returncode == 0 and "OK" in p.stdout, p.stdout + p.stderr
+
+
+def test_stager_error_in_the_middle_leaves_nothing_in_flight():
+    _fail_in_the_middle(capi.STAGE_LANES)
+
+
+@pytest.mark.parametrize("mode", [0, 3])      # slot streams, pageable bounce: the same chunk loop as the lanes
+def test_stager_error_in_the_middle_of_the_slot_and_bounce_pipelines(mode):
+    _fail_in_the_middle(mode)
 
 
 def test_cli_zero_arguments_is_the_reference_process():
