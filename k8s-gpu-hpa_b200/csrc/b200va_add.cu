@@ -108,11 +108,47 @@ int b200va::check_variant(int variant, unsigned flags)
 
 namespace {
 
-// ----------------------------------------------------------------------- vec dispatch
-// libb200va.so carries the production set only (what AUTO and the named variants resolve to,
-// plus close neighbours used by the parity tests); -DB200VA_TUNE_MATRIX (libb200va_tune.so, the
-// A/B tool's library) instantiates every combination of b200va_tune_t.  A combination that is
-// not compiled in makes the pick functions return nullptr -> B200VA_ERR_VARIANT.
+// ----------------------------------------------------------------------- kernel pick
+// What each library carries.  libb200va.so carries the production set: what AUTO and the named variants
+// resolve to, plus close neighbours the parity tests run.  -DB200VA_TUNE_MATRIX (libb200va_tune.so, the A/B
+// tool's library) carries every combination of b200va_tune_t.  The pick below instantiates exactly the
+// kernels these predicates admit; any other combination gives nullptr, and so B200VA_ERR_VARIANT.
+template <int VW, int UNROLL, int LD, int ST, int EARLY, int SCHED>
+constexpr bool carries_vec()
+{
+#ifdef B200VA_TUNE_MATRIX
+    return true;
+#else
+    if (SCHED == 1) return VW == 4 && LD == LD_PLAIN && ST == ST_NA && (UNROLL == 2 || UNROLL == 4);
+    return UNROLL <= 4 && (LD == LD_PLAIN || LD == LD_NA_EF) && (ST == ST_PLAIN || ST == ST_NA);
+#endif
+}
+
+// The static-split ring (store modes 0 and 1) is no production default: the production library keeps the
+// bulk-store (UBLKCP.G.S) form and one register-store form.  A bulk store takes no store hint, so store
+// mode 1 has its ST_PLAIN form only.
+template <int MODE, bool HINT, int ST>
+constexpr bool carries_tma()
+{
+    if (MODE == 1 && ST != ST_PLAIN) return false;
+#ifdef B200VA_TUNE_MATRIX
+    return true;
+#else
+    return !HINT && (MODE == 1 || ST == ST_NA);
+#endif
+}
+
+// K2d, the TMA production form: both load hints, plain and L1::no_allocate stores.
+template <bool HINT, int ST>
+constexpr bool carries_tma_dyn()
+{
+#ifdef B200VA_TUNE_MATRIX
+    return true;
+#else
+    return ST == ST_PLAIN || ST == ST_NA;
+#endif
+}
+
 using vec_fn = void (*)(const float*, const float*, float*, size_t, size_t, size_t, size_t);
 using dyn_fn = void (*)(const float*, const float*, float*, size_t, size_t, size_t, size_t, unsigned int*);
 
@@ -124,146 +160,46 @@ struct VecFn {
     const void* key() const { return plain ? reinterpret_cast<const void*>(plain) : reinterpret_cast<const void*>(dyn); }
 };
 
-template <int VW, int UNROLL, int LD, int ST>
-VecFn pick_early_hw(int early)
-{
-    VecFn f;
-    switch (early) {
-        case 0: f.plain = vadd_vec<VW, UNROLL, LD, ST, 0>; break;
-        case 1: f.plain = vadd_vec<VW, UNROLL, LD, ST, 1>; break;
-        case 2: f.plain = vadd_vec<VW, UNROLL, LD, ST, 2>; break;
-    }
-    return f;
-}
-
-template <int VW, int UNROLL, int LD, int ST>
-VecFn pick_early_dyn(int early)
-{
-    VecFn f;
-    switch (early) {
-        case 0: f.dyn = vadd_vec_dyn<VW, UNROLL, LD, ST, 0>; break;
-        case 1: f.dyn = vadd_vec_dyn<VW, UNROLL, LD, ST, 1>; break;
-        case 2: f.dyn = vadd_vec_dyn<VW, UNROLL, LD, ST, 2>; break;
-    }
-    return f;
-}
-
-template <int VW, int UNROLL, int LD, int ST>
-VecFn pick_sched(int early, int sched)
-{
-    if (sched == 1) {
-#ifdef B200VA_TUNE_MATRIX
-        return pick_early_dyn<VW, UNROLL, LD, ST>(early);
-#else
-        if constexpr (VW == 4 && LD == LD_PLAIN && ST == ST_NA && (UNROLL == 2 || UNROLL == 4))
-            return pick_early_dyn<VW, UNROLL, LD, ST>(early);
-        else
-            return VecFn{};
-#endif
-    }
-    return pick_early_hw<VW, UNROLL, LD, ST>(early);
-}
-
-template <int VW, int UNROLL, int LD>
-VecFn pick_st(int st, int early, int sched)
-{
-    switch (st) {
-        case ST_PLAIN: return pick_sched<VW, UNROLL, LD, ST_PLAIN>(early, sched);
-        case ST_NA:    return pick_sched<VW, UNROLL, LD, ST_NA>(early, sched);
-#ifdef B200VA_TUNE_MATRIX
-        case ST_CS:    return pick_sched<VW, UNROLL, LD, ST_CS>(early, sched);
-        case ST_NA_EF: return pick_sched<VW, UNROLL, LD, ST_NA_EF>(early, sched);
-#endif
-    }
-    return VecFn{};
-}
-
-template <int VW, int UNROLL>
-VecFn pick_ld(int ld, int st, int early, int sched)
-{
-    switch (ld) {
-        case LD_PLAIN: return pick_st<VW, UNROLL, LD_PLAIN>(st, early, sched);
-        case LD_NA_EF: return pick_st<VW, UNROLL, LD_NA_EF>(st, early, sched);
-#ifdef B200VA_TUNE_MATRIX
-        case LD_NA:    return pick_st<VW, UNROLL, LD_NA>(st, early, sched);
-        case LD_NC_NA: return pick_st<VW, UNROLL, LD_NC_NA>(st, early, sched);
-        case LD_CS:    return pick_st<VW, UNROLL, LD_CS>(st, early, sched);
-        case LD_NA_256: return pick_st<VW, UNROLL, LD_NA_256>(st, early, sched);
-#endif
-    }
-    return VecFn{};
-}
-
-template <int VW>
-VecFn pick_unroll(int unroll, int ld, int st, int early, int sched)
-{
-    switch (unroll) {
-        case 1: return pick_ld<VW, 1>(ld, st, early, sched);
-        case 2: return pick_ld<VW, 2>(ld, st, early, sched);
-        case 4: return pick_ld<VW, 4>(ld, st, early, sched);
-#ifdef B200VA_TUNE_MATRIX
-        case 8: return pick_ld<VW, 8>(ld, st, early, sched);
-#endif
-    }
-    return VecFn{};
-}
-
 VecFn pick_vec(int vw, int unroll, int ld, int st, int early, int sched)
 {
-    return vw == 8 ? pick_unroll<8>(unroll, ld, st, early, sched) : pick_unroll<4>(unroll, ld, st, early, sched);
+    VecFn f;
+    with_value<4, 8>(vw, [&](auto VW) {
+    with_value<1, 2, 4, 8>(unroll, [&](auto U) {
+    with_value<LD_PLAIN, LD_NA, LD_CS, LD_NA_EF, LD_NC_NA, LD_NA_256>(ld, [&](auto LD) {
+    with_value<ST_PLAIN, ST_NA, ST_CS, ST_NA_EF>(st, [&](auto ST) {
+    with_value<0, 1, 2>(early, [&](auto E) {
+    with_value<0, 1>(sched, [&](auto S) {
+        if constexpr (carries_vec<VW, U, LD, ST, E, S>()) {
+            if constexpr (S == 1) f.dyn = vadd_vec_dyn<VW, U, LD, ST, E>;
+            else f.plain = vadd_vec<VW, U, LD, ST, E>;
+        }
+    }); }); }); }); }); });
+    return f;
 }
 
-// ----------------------------------------------------------------------- tma dispatch
 using tma_fn = void (*)(const float*, const float*, float*, size_t, size_t, size_t, uint32_t, uint32_t);
 using tma_dyn_fn = void (*)(const float*, const float*, float*, size_t, size_t, size_t, uint32_t, uint32_t, unsigned int*);
 
-#ifdef B200VA_TUNE_MATRIX
-template <int MODE, bool HINT>
-tma_fn pick_tma_st(int st)
-{
-    switch (st) {
-        case ST_PLAIN: return vadd_tma<MODE, HINT, ST_PLAIN>;
-        case ST_NA:    return vadd_tma<MODE, HINT, ST_NA>;
-        case ST_CS:    return vadd_tma<MODE, HINT, ST_CS>;
-        case ST_NA_EF: return vadd_tma<MODE, HINT, ST_NA_EF>;
-    }
-    return nullptr;
-}
-#endif
-
-// store_mode 2: the dynamic tile scheduler, register stores
-template <bool HINT>
-tma_dyn_fn pick_tma_dyn_st(int st)
-{
-    switch (st) {
-        case ST_PLAIN: return vadd_tma_dyn<HINT, ST_PLAIN>;
-        case ST_NA:    return vadd_tma_dyn<HINT, ST_NA>;
-#ifdef B200VA_TUNE_MATRIX
-        case ST_CS:    return vadd_tma_dyn<HINT, ST_CS>;
-        case ST_NA_EF: return vadd_tma_dyn<HINT, ST_NA_EF>;
-#endif
-    }
-    return nullptr;
-}
-
-tma_dyn_fn pick_tma_dyn(bool l2_hint, int st)
-{
-    return l2_hint ? pick_tma_dyn_st<true>(st) : pick_tma_dyn_st<false>(st);
-}
-
 tma_fn pick_tma(int store_mode, bool l2_hint, int st)
 {
-#ifdef B200VA_TUNE_MATRIX
-    if (store_mode == 1)  // st hint is meaningless for bulk stores: one instantiation
-        return l2_hint ? vadd_tma<1, true, ST_PLAIN> : vadd_tma<1, false, ST_PLAIN>;
-    return l2_hint ? pick_tma_st<0, true>(st) : pick_tma_st<0, false>(st);
-#else
-    // the static-split ring (store modes 0/1) is not a production default: the tune library carries its
-    // matrix, this library two forms
-    if (store_mode == 1 && !l2_hint) return vadd_tma<1, false, ST_PLAIN>;   // kept: the bulk-store (UBLKCP.G.S) form
-    if (store_mode == 0 && !l2_hint && st == ST_NA) return vadd_tma<0, false, ST_NA>;
-    return nullptr;
-#endif
+    tma_fn f = nullptr;
+    with_value<0, 1>(store_mode, [&](auto M) {
+    with_value<0, 1>(l2_hint, [&](auto H) {
+    with_value<ST_PLAIN, ST_NA, ST_CS, ST_NA_EF>(M == 1 ? ST_PLAIN : st, [&](auto ST) {
+        if constexpr (carries_tma<M, H != 0, ST>()) f = vadd_tma<M, H != 0, ST>;
+    }); }); });
+    return f;
+}
+
+// store_mode 2: the dynamic tile scheduler, register stores
+tma_dyn_fn pick_tma_dyn(bool l2_hint, int st)
+{
+    tma_dyn_fn f = nullptr;
+    with_value<0, 1>(l2_hint, [&](auto H) {
+    with_value<ST_PLAIN, ST_NA, ST_CS, ST_NA_EF>(st, [&](auto ST) {
+        if constexpr (carries_tma_dyn<H != 0, ST>()) f = vadd_tma_dyn<H != 0, ST>;
+    }); });
+    return f;
 }
 
 // The tune b200va_add_f32_tuned runs for `in`: K_AUTO takes the whole AUTO tune for n, other zero
@@ -767,20 +703,11 @@ int b200va_host_fill_rand_f32(float* hA, float* hB, size_t n)
     return B200VA_OK;
 }
 
-static inline uint64_t host_splitmix64(uint64_t z)
-{
-    z += 0x9E3779B97F4A7C15ull;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
-}
-
 int b200va_host_fill_ctr_f32(float* h, size_t n, uint64_t seed, uint64_t first)
 {
     if (n && !h) return B200VA_ERR_INVALID;
     const uint64_t base = seed * 0x9E3779B97F4A7C15ull + first;
-    for (size_t i = 0; i < n; ++i)
-        h[i] = static_cast<float>(static_cast<uint32_t>(host_splitmix64(base + i) >> 40)) * 0x1.0p-24f;
+    for (size_t i = 0; i < n; ++i) h[i] = ctr_value(base + i);
     return B200VA_OK;
 }
 

@@ -15,6 +15,7 @@
 #include <cstring>
 #include <mutex>
 #include <new>
+#include <type_traits>
 
 #include "../../include/b200va.h"
 
@@ -88,6 +89,14 @@ int launch_kernel(void (*fn)(KArgs...), unsigned grid, unsigned block, size_t sm
     const cudaError_t e = cudaLaunchKernelEx(&cfg, fn, static_cast<KArgs>(args)...);
     if (e != cudaSuccess) cudaGetLastError();   // a refused launch must not stay latched for the next caller
     return cuda_err(e);
+}
+
+// Calls f(std::integral_constant<int, V>{}) for the V in Vs that equals v, and nothing if none does: turns a
+// runtime field into a template argument.  Nested calls pick a kernel from a tune.
+template <int... Vs, class F>
+void with_value(int v, F&& f)
+{
+    (void)((v == Vs && (f(std::integral_constant<int, Vs>{}), true)) || ...);
 }
 
 // ---- the rules the f32 add and the STREAM ops share

@@ -237,9 +237,50 @@ __global__ void vadd_vec_dyn(const float* A, const float* B, float* C, size_t n,
     if (threadIdx.x == 0) sched_retire(sched);
 }
 
+// ------------------------------------------------------------------------------ K2 / K2d ring
+// Shared memory: [stages][A tile | B tile] then full[stages], empty[stages] mbarriers (K2d adds a tile
+// slot per stage after them).  Warp 0 lane 0 = producer, warps 1.. = consumers (blockDim.x - 32 threads).
+struct TmaRing {
+    uint32_t base, bars, stages, tile_bytes;
+
+    __device__ TmaRing(const unsigned char* smem, uint32_t stages_, uint32_t tile_bytes_)
+        : base(smem_u32(smem)), bars(base + stages_ * 2u * tile_bytes_), stages(stages_), tile_bytes(tile_bytes_) {}
+    __device__ uint32_t full(uint32_t s) const { return bars + s * 8u; }
+    __device__ uint32_t empty(uint32_t s) const { return bars + (stages + s) * 8u; }
+    __device__ uint32_t tile_a(uint32_t s) const { return base + s * 2u * tile_bytes; }
+    __device__ uint32_t tile_b(uint32_t s) const { return base + s * 2u * tile_bytes + tile_bytes; }
+    // The tile at byte `off` of a `body`-byte vector body: a whole tile, or the rest of the body.
+    __device__ uint32_t bytes(size_t off, size_t body) const
+    {
+        const size_t left = body - off;
+        return left < tile_bytes ? static_cast<uint32_t>(left) : tile_bytes;
+    }
+    // full[s] completes on the producer's arrive and its bytes, empty[s] on `empty_count` arrivals.
+    __device__ void init(uint32_t empty_count) const
+    {
+        if (threadIdx.x == 0) {
+            for (uint32_t s = 0; s < stages; ++s) {
+                mbar_init(full(s), 1u);
+                mbar_init(empty(s), empty_count);
+            }
+            mbar_fence_init();
+            fence_proxy_async_smem();
+        }
+        __syncthreads();
+    }
+    // The producer: the A and B tiles at byte `off` into stage s, counted on full[s].
+    template <bool L2_HINT>
+    __device__ void load(uint32_t s, const unsigned char* a, const unsigned char* b, size_t off, uint32_t bytes,
+                         uint64_t pol) const
+    {
+        mbar_arrive_expect_tx(full(s), 2u * bytes);
+        bulk_g2s<L2_HINT>(tile_a(s), a + off, bytes, full(s), pol);
+        bulk_g2s<L2_HINT>(tile_b(s), b + off, bytes, full(s), pol);
+    }
+};
+
 // ------------------------------------------------------------------------------ K2
-// Shared memory: [stages][A tile | B tile] then full[stages], empty[stages] mbarriers.
-// Warp 0 lane 0 = producer, warps 1.. = consumers (blockDim.x - 32 threads).
+// The ring with a static persistent split: CTA i takes tiles i, i + gridDim.x, ...
 //   STORE_MODE 0: consumers ld.shared both tiles, add, st.global.v4 from registers;
 //                 every consumer warp arrives on empty[s] when done reading.
 //   STORE_MODE 1: consumers write the sum in place over the A tile, fence to the async
@@ -252,25 +293,9 @@ vadd_tma(const float* A, const float* B, float* C, size_t n, size_t head, size_t
          uint32_t tile_bytes, uint32_t stages)
 {
     extern __shared__ __align__(128) unsigned char smem[];
-    const uint32_t smem_base = smem_u32(smem);
-    const uint32_t bar_base = smem_base + stages * 2u * tile_bytes;
+    const TmaRing ring(smem, stages, tile_bytes);
     const uint32_t n_cons = blockDim.x - 32u;
-    const uint32_t n_cons_warps = n_cons >> 5;
-
-    auto full_bar = [&](uint32_t s) { return bar_base + s * 8u; };
-    auto empty_bar = [&](uint32_t s) { return bar_base + (stages + s) * 8u; };
-    auto tile_a = [&](uint32_t s) { return smem_base + s * 2u * tile_bytes; };
-    auto tile_b = [&](uint32_t s) { return smem_base + s * 2u * tile_bytes + tile_bytes; };
-
-    if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < stages; ++s) {
-            mbar_init(full_bar(s), 1u);
-            mbar_init(empty_bar(s), STORE_MODE == 0 ? n_cons_warps : 1u);
-        }
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    __syncthreads();
+    ring.init(STORE_MODE == 0 ? n_cons >> 5 : 1u);
 
     const unsigned char* a = reinterpret_cast<const unsigned char*>(A + head);
     const unsigned char* b = reinterpret_cast<const unsigned char*>(B + head);
@@ -288,13 +313,9 @@ vadd_tma(const float* A, const float* B, float* C, size_t n, size_t head, size_t
         if (threadIdx.x == 0) {
             uint32_t s = 0, ph = 0;
             for (size_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
-                mbar_wait(empty_bar(s), ph ^ 1u);
+                mbar_wait(ring.empty(s), ph ^ 1u);
                 const size_t off = t * tile_bytes;
-                const size_t left = body_bytes - off;
-                const uint32_t bytes = left < tile_bytes ? static_cast<uint32_t>(left) : tile_bytes;
-                mbar_arrive_expect_tx(full_bar(s), 2u * bytes);
-                bulk_g2s<L2_HINT>(tile_a(s), a + off, bytes, full_bar(s), pol);
-                bulk_g2s<L2_HINT>(tile_b(s), b + off, bytes, full_bar(s), pol);
+                ring.load<L2_HINT>(s, a, b, off, ring.bytes(off, body_bytes), pol);
                 if (++s == stages) { s = 0; ph ^= 1u; }
             }
         }
@@ -304,12 +325,11 @@ vadd_tma(const float* A, const float* B, float* C, size_t n, size_t head, size_t
         uint32_t s = 0, ph = 0, prev_s = 0;
         bool have_prev = false;
         for (size_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
-            mbar_wait(full_bar(s), ph);
+            mbar_wait(ring.full(s), ph);
             const size_t off = t * tile_bytes;
-            const size_t left = body_bytes - off;
-            const uint32_t bytes = left < tile_bytes ? static_cast<uint32_t>(left) : tile_bytes;
+            const uint32_t bytes = ring.bytes(off, body_bytes);
             const uint32_t nv = bytes >> 4;
-            const uint32_t sa = tile_a(s), sb = tile_b(s);
+            const uint32_t sa = ring.tile_a(s), sb = ring.tile_b(s);
 
             uint32_t v = ct;
             for (; v + 3u * n_cons < nv; v += 4u * n_cons) {
@@ -337,7 +357,7 @@ vadd_tma(const float* A, const float* B, float* C, size_t n, size_t head, size_t
 
             if constexpr (STORE_MODE == 0) {
                 __syncwarp();
-                if ((threadIdx.x & 31u) == 0) mbar_arrive(empty_bar(s));
+                if ((threadIdx.x & 31u) == 0) mbar_arrive(ring.empty(s));
             } else {
                 fence_proxy_async_smem();
                 named_bar_sync(1, n_cons);
@@ -346,7 +366,7 @@ vadd_tma(const float* A, const float* B, float* C, size_t n, size_t head, size_t
                     bulk_commit();
                     if (have_prev) {
                         bulk_wait_read<1>();
-                        mbar_arrive(empty_bar(prev_s));
+                        mbar_arrive(ring.empty(prev_s));
                     }
                 }
                 prev_s = s;
@@ -374,28 +394,12 @@ vadd_tma_dyn(const float* A, const float* B, float* C, size_t n, size_t head, si
              uint32_t tile_bytes, uint32_t stages, unsigned int* sched)
 {
     extern __shared__ __align__(128) unsigned char smem[];
-    const uint32_t smem_base = smem_u32(smem);
-    const uint32_t bar_base = smem_base + stages * 2u * tile_bytes;       // full[], empty[]
-    const uint32_t slot_base = bar_base + 2u * stages * 8u;               // uint32 tile index per stage
+    const TmaRing ring(smem, stages, tile_bytes);
     const uint32_t n_cons = blockDim.x - 32u;
-    const uint32_t n_cons_warps = n_cons >> 5;
     constexpr uint32_t kDone = 0xffffffffu;
-
-    auto full_bar = [&](uint32_t s) { return bar_base + s * 8u; };
-    auto empty_bar = [&](uint32_t s) { return bar_base + (stages + s) * 8u; };
-    auto tile_a = [&](uint32_t s) { return smem_base + s * 2u * tile_bytes; };
-    auto tile_b = [&](uint32_t s) { return smem_base + s * 2u * tile_bytes + tile_bytes; };
-    volatile uint32_t* tile_slot = reinterpret_cast<volatile uint32_t*>(smem + (slot_base - smem_base));
-
-    if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < stages; ++s) {
-            mbar_init(full_bar(s), 1u);
-            mbar_init(empty_bar(s), n_cons_warps);
-        }
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    __syncthreads();
+    // uint32 tile index per stage, after the barriers
+    volatile uint32_t* tile_slot = reinterpret_cast<volatile uint32_t*>(smem + (ring.bars + 2u * stages * 8u - ring.base));
+    ring.init(n_cons >> 5);
 
     const unsigned char* a = reinterpret_cast<const unsigned char*>(A + head);
     const unsigned char* b = reinterpret_cast<const unsigned char*>(B + head);
@@ -413,19 +417,16 @@ vadd_tma_dyn(const float* A, const float* B, float* C, size_t n, size_t head, si
             // ---------------------------------------------------- producer + scheduler
             uint32_t s = 0, ph = 0;
             for (size_t tile = blockIdx.x; tile < ntiles; tile = sched_next_tile(sched)) {
-                mbar_wait(empty_bar(s), ph ^ 1u);
+                mbar_wait(ring.empty(s), ph ^ 1u);
                 const size_t off = tile * tile_bytes;
-                const size_t left = body_bytes - off;
-                const uint32_t bytes = left < tile_bytes ? static_cast<uint32_t>(left) : tile_bytes;
+                const uint32_t bytes = ring.bytes(off, body_bytes);
                 tile_slot[s] = static_cast<uint32_t>(tile);       // published by the arrive below (release)
-                mbar_arrive_expect_tx(full_bar(s), 2u * bytes);
-                bulk_g2s<L2_HINT>(tile_a(s), a + off, bytes, full_bar(s), pol);
-                bulk_g2s<L2_HINT>(tile_b(s), b + off, bytes, full_bar(s), pol);
+                ring.load<L2_HINT>(s, a, b, off, bytes, pol);
                 if (++s == stages) { s = 0; ph ^= 1u; }
             }
-            mbar_wait(empty_bar(s), ph ^ 1u);                     // sentinel: no more tiles
+            mbar_wait(ring.empty(s), ph ^ 1u);                    // sentinel: no more tiles
             tile_slot[s] = kDone;
-            mbar_arrive(full_bar(s));
+            mbar_arrive(ring.full(s));
             sched_retire(sched);
         }
     } else {
@@ -433,14 +434,12 @@ vadd_tma_dyn(const float* A, const float* B, float* C, size_t n, size_t head, si
         const uint32_t ct = threadIdx.x - 32u;
         uint32_t s = 0, ph = 0;
         while (true) {
-            mbar_wait(full_bar(s), ph);
+            mbar_wait(ring.full(s), ph);
             const uint32_t tile = tile_slot[s];
             if (tile == kDone) break;
             const size_t off = static_cast<size_t>(tile) * tile_bytes;
-            const size_t left = body_bytes - off;
-            const uint32_t bytes = left < tile_bytes ? static_cast<uint32_t>(left) : tile_bytes;
-            const uint32_t nv = bytes >> 4;
-            const uint32_t sa = tile_a(s), sb = tile_b(s);
+            const uint32_t nv = ring.bytes(off, body_bytes) >> 4;
+            const uint32_t sa = ring.tile_a(s), sb = ring.tile_b(s);
             float* cg = reinterpret_cast<float*>(c + off);
 
             uint32_t v = ct;
@@ -456,7 +455,7 @@ vadd_tma_dyn(const float* A, const float* B, float* C, size_t n, size_t head, si
             for (; v < nv; v += n_cons)
                 stg128<ST>(cg + v * 4u, add_vec(lds128(sa + v * 16u), lds128(sb + v * 16u)), pol);
             __syncwarp();
-            if ((threadIdx.x & 31u) == 0) mbar_arrive(empty_bar(s));
+            if ((threadIdx.x & 31u) == 0) mbar_arrive(ring.empty(s));
             if (++s == stages) { s = 0; ph ^= 1u; }
         }
         // the scalar head/tail: CTA 0 always runs tile 0, and exists even when there is no vector body
@@ -498,39 +497,36 @@ __global__ void probe_copy(const float* A, float* C, size_t nvec)
 }
 
 // ---------------------------------------------------------------- support kernels
-__device__ __forceinline__ uint64_t splitmix64(uint64_t z)
+// a2, the counter generator: element i is ctr_value(base + i), base = seed * 0x9E3779B97F4A7C15 + first.
+// One definition for the host (b200va_host_fill_ctr_f32) and the device (fill_ctr, fill_ctr_vec).  A 24-bit
+// integer converts to binary32 exactly and the scale is a power of two, so both give the same bits.
+__host__ __device__ __forceinline__ float ctr_value(uint64_t z)
 {
-    z += 0x9E3779B97F4A7C15ull;
+    z += 0x9E3779B97F4A7C15ull;                       // splitmix64
     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
     z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
+    z ^= z >> 31;
+    return static_cast<float>(static_cast<uint32_t>(z >> 40)) * 0x1.0p-24f;
 }
 
-// a2 for the large configs: x[i] = (float)(splitmix64(base + i) >> 40) * 2^-24.
-// A 24-bit integer converts to binary32 exactly and the scale is a power of two, so the
-// device values are bit-identical to the host generator by construction.
 __global__ void fill_ctr(float* x, size_t n, uint64_t base)
 {
     const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
     for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride)
-        x[i] = __uint2float_rn(static_cast<uint32_t>(splitmix64(base + i) >> 40)) * 0x1.0p-24f;
+        x[i] = ctr_value(base + i);
 }
 
 // 128-bit form for 16-byte-aligned x: thread v generates elements 4v..4v+3 and stores them with one STG.128;
-// the < 4-element tail is written by the first threads of CTA 0.  Same values as fill_ctr by construction.
+// the < 4-element tail is written by the first threads of CTA 0.
 __global__ void fill_ctr_vec(float* x, size_t n, uint64_t base)
 {
     const size_t nvec = n / 4, stride = static_cast<size_t>(gridDim.x) * blockDim.x;
     for (size_t v = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; v < nvec; v += stride) {
-        f32x4 r;
-        r.x = __uint2float_rn(static_cast<uint32_t>(splitmix64(base + 4 * v + 0) >> 40)) * 0x1.0p-24f;
-        r.y = __uint2float_rn(static_cast<uint32_t>(splitmix64(base + 4 * v + 1) >> 40)) * 0x1.0p-24f;
-        r.z = __uint2float_rn(static_cast<uint32_t>(splitmix64(base + 4 * v + 2) >> 40)) * 0x1.0p-24f;
-        r.w = __uint2float_rn(static_cast<uint32_t>(splitmix64(base + 4 * v + 3) >> 40)) * 0x1.0p-24f;
+        const f32x4 r{ctr_value(base + 4 * v + 0), ctr_value(base + 4 * v + 1), ctr_value(base + 4 * v + 2),
+                      ctr_value(base + 4 * v + 3)};
         stg128<ST_NA>(x + 4 * v, r, 0);
     }
-    if (blockIdx.x == 0 && 4 * nvec + threadIdx.x < n)
-        x[4 * nvec + threadIdx.x] = __uint2float_rn(static_cast<uint32_t>(splitmix64(base + 4 * nvec + threadIdx.x) >> 40)) * 0x1.0p-24f;
+    if (blockIdx.x == 0 && 4 * nvec + threadIdx.x < n) x[4 * nvec + threadIdx.x] = ctr_value(base + 4 * nvec + threadIdx.x);
 }
 
 __device__ __forceinline__ bool is_nan_bits(uint32_t u) { return (u & 0x7fffffffu) > 0x7f800000u; }

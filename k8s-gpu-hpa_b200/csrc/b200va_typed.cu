@@ -15,6 +15,18 @@ size_t dtype_size(int dtype) { return dtype == DT_F64 ? 8 : dtype == DT_F32 ? 4 
 // a vector body peels off.
 size_t head_peel(uintptr_t a, size_t es) { return ((16u - (a & 15u)) & 15u) / es; }
 
+// The stream_vec forms each library carries (every DT): the production library only the two plain forms and
+// the ST_NA form the HBM class picks, the tune library every form B200VA_STREAM_GEOMETRY can ask for.
+template <int OP, int UNROLL, int ST>
+constexpr bool carries_stream()
+{
+#ifdef B200VA_TUNE_MATRIX
+    return true;
+#else
+    return UNROLL <= 2 && (ST == ST_PLAIN || UNROLL == (OP == OP_ADD || OP == OP_TRIAD ? 1 : 2));
+#endif
+}
+
 template <int DT, int OP>
 int launch_stream_typed(const void* dA, const void* dB, void* dC, size_t n, double scalar, cudaStream_t st)
 {
@@ -38,14 +50,13 @@ int launch_stream_typed(const void* dA, const void* dB, void* dC, size_t n, doub
     const size_t m = n * ES / 4;
     const bool hbm = hbm_class(n, ES);
     unsigned threads = 128;
-    int unroll = 1;
-    bool skip_l1_stores = false;
+    int unroll = 1, st_hint = ST_PLAIN;
     if (hbm) {
         // three-array ops like the add: 512 x 1; two-array ops (copy, scale) want twice the bytes in
-        // flight per thread: 1024 x 2
+        // flight per thread: 1024 x 2; stores skip L1
         threads = binary ? 512 : 1024;
         unroll = binary ? 1 : 2;
-        skip_l1_stores = true;
+        st_hint = ST_NA;
     } else if (m > (size_t{1} << 23)) { threads = 128; unroll = 2; }
     else if (m >= (size_t{1} << 21)) { threads = 256; unroll = 2; }
     else if (m >= (size_t{1} << 19)) { threads = 512; }
@@ -59,7 +70,7 @@ int launch_stream_typed(const void* dA, const void* dB, void* dC, size_t n, doub
     if (ov.threads >= 32 && ov.threads <= 1024 && (ov.threads & 31) == 0 && (ov.unroll == 1 || ov.unroll == 2 || ov.unroll == 4)) {
         threads = static_cast<unsigned>(ov.threads);
         unroll = ov.unroll;
-        skip_l1_stores = ov.na != 0;
+        st_hint = ov.na ? ST_NA : ST_PLAIN;
     }
 #endif
     const size_t tile_vecs = static_cast<size_t>(threads) * unroll;
@@ -68,30 +79,12 @@ int launch_stream_typed(const void* dA, const void* dB, void* dC, size_t n, doub
     using fn_t = void (*)(const void*, const void*, void*, size_t, size_t, size_t, size_t, S, int);
     const int prefetch_first = hbm ? 1 : 0;
     fn_t fn = nullptr;
-#ifdef B200VA_TUNE_MATRIX
-    if (unroll == 4) fn = skip_l1_stores ? stream_vec<DT, OP, 4, LD_PLAIN, ST_NA> : stream_vec<DT, OP, 4, LD_PLAIN, ST_PLAIN>;
-    else if (skip_l1_stores) fn = unroll == 2 ? stream_vec<DT, OP, 2, LD_PLAIN, ST_NA> : stream_vec<DT, OP, 1, LD_PLAIN, ST_NA>;
-#else
-    // the production library carries only the ST_NA form the HBM class above picks
-    if (skip_l1_stores) {
-        if constexpr (binary) fn = stream_vec<DT, OP, 1, LD_PLAIN, ST_NA>;
-        else fn = stream_vec<DT, OP, 2, LD_PLAIN, ST_NA>;
-    }
-#endif
-    if (!fn) fn = unroll == 2 ? stream_vec<DT, OP, 2, LD_PLAIN, ST_PLAIN> : stream_vec<DT, OP, 1, LD_PLAIN, ST_PLAIN>;
+    with_value<1, 2, 4>(unroll, [&](auto U) {
+    with_value<ST_PLAIN, ST_NA>(st_hint, [&](auto ST) {
+        if constexpr (carries_stream<OP, U, ST>()) fn = stream_vec<DT, OP, U, LD_PLAIN, ST>;
+    }); });
+    if (!fn) return B200VA_ERR_VARIANT;
     return launch_kernel(fn, static_cast<unsigned>(grid), threads, 0, st, pdl_enabled(), dA, dB, dC, n, head, nvec, ntiles, s, prefetch_first);
-}
-
-template <int DT>
-int launch_stream_op(int op, const void* dA, const void* dB, void* dC, size_t n, double scalar, cudaStream_t st)
-{
-    switch (op) {
-        case OP_COPY:  return launch_stream_typed<DT, OP_COPY>(dA, dB, dC, n, scalar, st);
-        case OP_SCALE: return launch_stream_typed<DT, OP_SCALE>(dA, dB, dC, n, scalar, st);
-        case OP_ADD:   return launch_stream_typed<DT, OP_ADD>(dA, dB, dC, n, scalar, st);
-        case OP_TRIAD: return launch_stream_typed<DT, OP_TRIAD>(dA, dB, dC, n, scalar, st);
-    }
-    return B200VA_ERR_VARIANT;
 }
 
 // Pass 1 of b200va_dot: one CTA per chunk, one f64 partial each into ws.  The vector form when A and
@@ -121,14 +114,12 @@ int b200va_stream(int op, int dtype, const void* dA, const void* dB, void* dC, s
     RC_TRY(current_dev_info(nullptr));
     RC_TRY(check_operands(dtype_size(dtype), dA, dB, dC, n, op == OP_ADD || op == OP_TRIAD));
     if (n == 0) return B200VA_OK;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    switch (dtype) {
-        case DT_F32:  return launch_stream_op<DT_F32>(op, dA, dB, dC, n, scalar, st);
-        case DT_F64:  return launch_stream_op<DT_F64>(op, dA, dB, dC, n, scalar, st);
-        case DT_F16:  return launch_stream_op<DT_F16>(op, dA, dB, dC, n, scalar, st);
-        case DT_BF16: return launch_stream_op<DT_BF16>(op, dA, dB, dC, n, scalar, st);
-    }
-    return B200VA_ERR_VARIANT;
+    int rc = B200VA_ERR_VARIANT;
+    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dtype, [&](auto DT) {
+    with_value<OP_COPY, OP_SCALE, OP_ADD, OP_TRIAD>(op, [&](auto OP) {
+        rc = launch_stream_typed<DT, OP>(dA, dB, dC, n, scalar, static_cast<cudaStream_t>(stream));
+    }); });
+    return rc;
 }
 
 size_t b200va_dot_workspace_bytes(size_t n)
@@ -157,14 +148,9 @@ int b200va_dot(int dtype, const void* dA, const void* dB, size_t n, double* d_ou
         return B200VA_ERR_OVERLAP;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     double* ws = static_cast<double*>(d_workspace);
-    if (n) {
-        switch (dtype) {
-            case DT_F32:  RC_TRY(launch_dot_typed<DT_F32>(dA, dB, n, ws, st)); break;
-            case DT_F64:  RC_TRY(launch_dot_typed<DT_F64>(dA, dB, n, ws, st)); break;
-            case DT_F16:  RC_TRY(launch_dot_typed<DT_F16>(dA, dB, n, ws, st)); break;
-            case DT_BF16: RC_TRY(launch_dot_typed<DT_BF16>(dA, dB, n, ws, st)); break;
-        }
-    }
+    int rc = B200VA_OK;
+    if (n) with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dtype, [&](auto DT) { rc = launch_dot_typed<DT>(dA, dB, n, ws, st); });
+    RC_TRY(rc);
     // pass 2: aligned blocks of DOT_FINAL_BLOCK partials per CTA, one level per launch, until one CTA
     // writes *d_out (for n = 0 it sums nothing and writes +0.0)
     size_t k = need / 8, stride = 1;
