@@ -275,6 +275,19 @@ int b200va_device_numa_node_of(int device);
 int b200va_stream(int op, int dtype, const void *dA, const void *dB, void *dC, size_t n,
                   double scalar, void *stream);
 
+/* c[i] = a[i] rounded once to dst_dtype (B200VA_DT_* codes on both sides): IEEE round-to-
+ * nearest-even as if the exponent range were unbounded, then overflow to +-inf.  No FTZ on
+ * either side: subnormal inputs and results stay.  Widening is exact; +-0 and +-inf are kept;
+ * a NaN gives a NaN (payload and sign unspecified).  f16 <-> bf16 widen exactly to f32 and round
+ * once; f64 -> f16/bf16 never goes through f32.  src_dtype == dst_dtype is a bit copy, NaN
+ * payloads included (the COPY of b200va_stream).
+ * B200VA_ERR_VARIANT: bad dtype code.  B200VA_ERR_INVALID: NULL dA/dC with n > 0, n > 2^40.
+ * B200VA_ERR_ALIGN: a pointer not aligned to its own element size.  B200VA_ERR_OVERLAP: C meets A
+ * anywhere, except dC == dA when both element sizes are equal (the same type, f16 <-> bf16).
+ * Asynchronous on `stream`: one kernel launch, no allocation, synchronisation or memset;
+ * capturable in a CUDA graph. */
+int b200va_convert(int src_dtype, const void *dA, int dst_dtype, void *dC, size_t n, void *stream);
+
 /* ---- reproducible dot product (row f4) --------------------------------------------------
  * *d_out = sum_i a_i b_i as a binary64 value in device memory, written asynchronously on `stream`
  * (not rounded to the storage type; dtype is a B200VA_DT_* code).  Every operand is widened

@@ -108,6 +108,7 @@ _SIGS = {
     "b200va_device_numa_node": (_I, []),
     "b200va_device_numa_node_of": (_I, [_I]),
     "b200va_stream": (_I, [_I, _I, _P, _P, _P, _SZ, C.c_double, _P]),
+    "b200va_convert": (_I, [_I, _P, _I, _P, _SZ, _P]),
     "b200va_dot_workspace_bytes": (_SZ, [_SZ]),
     "b200va_dot": (_I, [_I, _P, _P, _SZ, _P, _P, _SZ, _P]),
     "b200va_probe_f32": (_I, [_I, _P, _P, _P, _SZ, _P]),

@@ -120,6 +120,21 @@ inline int check_operands(size_t es, const void* pa, const void* pb, const void*
     return B200VA_OK;
 }
 
+// C = convert(A), A of `esa`-byte and C of `esc`-byte elements: the rules of check_operands, except that
+// operands of different element sizes must not meet at all.  With exact aliasing the wide side's stores
+// would overwrite elements of the narrow side that other threads have not read yet.
+inline int check_convert_operands(size_t esa, const void* pa, size_t esc, const void* pc, size_t n)
+{
+    if (esa == esc) return check_operands(esa, pa, nullptr, pc, n, false);
+    if (n == 0) return B200VA_OK;
+    if (!pa || !pc) return B200VA_ERR_INVALID;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(pa), c = reinterpret_cast<uintptr_t>(pc);
+    if ((a & (esa - 1)) || (c & (esc - 1))) return B200VA_ERR_ALIGN;
+    if (n > (size_t{1} << 40)) return B200VA_ERR_INVALID;
+    if (a < c + n * esc && c < a + n * esa) return B200VA_ERR_OVERLAP;
+    return B200VA_OK;
+}
+
 // ---- b200va_add.cu: the f32 add, as the host-buffer stager calls it
 void default_tune(int variant, size_t n, b200va_tune_t* t, unsigned flags = 0);
 int check_variant(int variant, unsigned flags = 0);

@@ -1,7 +1,8 @@
-// b200va_typed.cu -- the STREAM ops (copy, scale, add, triad) and the reproducible dot product over
-// f32, f64, f16 and bf16.  The only unit that includes the STREAM and dot kernels (b200va_dot.cuh,
-// which includes b200va_stream.cuh).
+// b200va_typed.cu -- the STREAM ops (copy, scale, add, triad), the reproducible dot product and the
+// conversions between f32, f64, f16 and bf16.  The only unit that includes the STREAM, dot and convert
+// kernels (b200va_dot.cuh and b200va_convert.cuh, which include b200va_stream.cuh).
 #include "b200va_internal.h"
+#include "b200va_convert.cuh"
 #include "b200va_dot.cuh"
 
 using namespace b200va;
@@ -104,6 +105,32 @@ int launch_dot_typed(const void* dA, const void* dB, size_t n, double* ws, cudaS
                          ws, prefetch_first);
 }
 
+// b200va_convert between two distinct types: one convert_vec launch.  The head is the smallest h < G at
+// which A and C both sit on a 16-byte boundary; with none (mixed phase) head = n, and the kernel's scalar
+// loop takes every element.  The geometry is one form for the HBM class (the wider operand >= 128 MiB) and
+// one below it, neither measured yet.
+template <int SRC, int DST>
+int launch_convert_typed(const void* dA, void* dC, size_t n, cudaStream_t st)
+{
+    using S = convert_shape<SRC, DST>;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC);
+    size_t head = n;
+    for (size_t h = head_peel(a, S::ESS); h < static_cast<size_t>(S::G); h += 16 / S::ESS)
+        if (((c + h * S::ESD) & 15u) == 0) { head = h; break; }
+    if (head > n) head = n;
+    const size_t ngroups = (n - head) / S::G;
+    const size_t edges = n - ngroups * S::G;
+    const bool hbm = hbm_class(n, std::max(S::ESS, S::ESD));
+    const unsigned threads = hbm ? 512 : 256;
+    const int unroll = hbm ? 2 : 1;
+    const int prefetch_first = hbm ? 1 : 0;
+    const size_t tile = static_cast<size_t>(threads) * unroll;
+    const size_t blocks = std::max((ngroups + tile - 1) / tile, (edges + threads - 1) / threads);
+    const unsigned grid = static_cast<unsigned>(std::max<size_t>(std::min<size_t>(blocks, 0x7fffffff), 1));
+    return launch_kernel(convert_vec<SRC, DST>, grid, threads, 0, st, pdl_enabled(), dA, dC, n, head, ngroups, unroll,
+                         prefetch_first);
+}
+
 }  // namespace
 
 // ========================================= ABI (C linkage from the declarations in include/b200va.h)
@@ -119,6 +146,23 @@ int b200va_stream(int op, int dtype, const void* dA, const void* dB, void* dC, s
     with_value<OP_COPY, OP_SCALE, OP_ADD, OP_TRIAD>(op, [&](auto OP) {
         rc = launch_stream_typed<DT, OP>(dA, dB, dC, n, scalar, static_cast<cudaStream_t>(stream));
     }); });
+    return rc;
+}
+
+int b200va_convert(int src_dtype, const void* dA, int dst_dtype, void* dC, size_t n, void* stream)
+{
+    if (src_dtype < 0 || src_dtype >= DT_COUNT || dst_dtype < 0 || dst_dtype >= DT_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    RC_TRY(check_convert_operands(dtype_size(src_dtype), dA, dtype_size(dst_dtype), dC, n));
+    if (n == 0) return B200VA_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int rc = B200VA_ERR_VARIANT;
+    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(src_dtype, [&](auto SRC) {
+        if (src_dtype == dst_dtype) { rc = launch_stream_typed<SRC, OP_COPY>(dA, nullptr, dC, n, 0.0, st); return; }
+        with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dst_dtype, [&](auto DST) {
+            if constexpr (SRC != DST) rc = launch_convert_typed<SRC, DST>(dA, dC, n, st);
+        });
+    });
     return rc;
 }
 

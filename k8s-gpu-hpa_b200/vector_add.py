@@ -135,6 +135,32 @@ def stream(op: str, a, b=None, out=None, *, scalar: float = 0.0, stream=None):
     return out
 
 
+def convert(a, dtype, out=None, *, stream=None):
+    """``a`` rounded once to ``dtype`` (torch.float32/float64/float16/bfloat16, or "f32"/"f64"/"f16"/"bf16")
+    through b200va_convert: round-to-nearest-even, no FTZ, overflow to inf; the same dtype is a bit copy.
+    ``out``: a contiguous CUDA tensor of ``dtype`` with a's length on a's device (it may be ``a`` itself when
+    both element sizes are equal), else a new one.  Asynchronous on the current stream."""
+    torch = _torch()
+    names = {getattr(torch, v): k for k, v in _TORCH_DT.items()}
+    if not isinstance(a, torch.Tensor) or not a.is_cuda or a.dtype not in names or not a.is_contiguous():
+        raise TypeError("a must be a contiguous CUDA tensor of float32/float64/float16/bfloat16")
+    if isinstance(dtype, str):
+        if dtype not in _TORCH_DT:
+            raise TypeError(f"dtype must be one of {sorted(_TORCH_DT)}, got {dtype!r}")
+        dtype = getattr(torch, _TORCH_DT[dtype])
+    if dtype not in names:
+        raise TypeError(f"dtype must be float32/float64/float16/bfloat16, got {dtype}")
+    if out is None:
+        out = torch.empty(a.shape, dtype=dtype, device=a.device)
+    elif (not isinstance(out, torch.Tensor) or out.dtype != dtype or out.numel() != a.numel() or out.device != a.device
+          or not out.is_contiguous()):
+        raise TypeError("out must be a contiguous tensor of dtype with a's length on a's device")
+    with torch.cuda.device(a.device):
+        check(lib.b200va_convert(capi.DTYPES[names[a.dtype]], a.data_ptr(), capi.DTYPES[names[dtype]], out.data_ptr(),
+                                 a.numel(), _stream_ptr(stream)), "b200va_convert")
+    return out
+
+
 def dot(a, b, *, out=None, workspace=None, stream=None):
     """The reproducible dot product of two equal-length contiguous CUDA tensors of one of f32/f64/f16/bf16
     (b200va_dot): a 0-d float64 CUDA tensor, written asynchronously on the current stream.  The bits
