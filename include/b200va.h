@@ -137,8 +137,10 @@ int b200va_add_f32_tuned(const float *dA, const float *dB, float *dC, size_t n,
  * one on `stream` does not write A or B (e.g. it is another add into a different or the
  * same C).  The kernel then issues its loads while that launch is still draining and only
  * its stores wait for it (programmatic dependent launch), which removes most of the
- * ~2 us bubble between back-to-back launches.  Results and stream order of C are
- * unchanged; the flag is ignored when C aliases A or B. */
+ * ~2 us bubble between back-to-back launches.  The library's kernels release their
+ * successor only after their own wait, so the immediately preceding launch is the only
+ * one that can still be running.  Results and stream order of C are unchanged; the flag
+ * is ignored when C aliases A or B. */
 #define B200VA_F_INPUTS_STABLE 1u
 /* B200VA_F_COLD: the operands are not L2-resident (fresh from a copy engine, or one of many
  * buffer sets touched in rotation): B200VA_K_AUTO then resolves to the geometry tuned on

@@ -170,7 +170,6 @@ __global__ void convert_vec(const void* A, void* C, size_t n, size_t head, size_
     using S = convert_shape<SRC, DST>;
     const unsigned char* a = static_cast<const unsigned char*>(A);
     unsigned char* c = static_cast<unsigned char*>(C);
-    pdl_launch_dependents();
     if (prefetch_first && threadIdx.x == 0) {
         const size_t tile = static_cast<size_t>(blockDim.x) * unroll, g0 = blockIdx.x * tile;
         if (g0 < ngroups)

@@ -160,7 +160,6 @@ dot_vec(const void* A, const void* B, size_t n, size_t head, double* partials, i
     const unsigned char* a = static_cast<const unsigned char*>(A) + base * ES;
     const unsigned char* b = static_cast<const unsigned char*>(B) + base * ES;
     const int e0 = head ? static_cast<int>(head) - EPV : 0;
-    pdl_launch_dependents();
     if (prefetch_first && threadIdx.x == 0) dot_prefetch(a, b, static_cast<size_t>(len) * ES, size_t{ROWS} * DOT_LANES * ES);
     pdl_wait();
 
@@ -234,7 +233,6 @@ dot_scalar(const void* A, const void* B, size_t n, double* partials, int prefetc
     const int len = n - base < static_cast<size_t>(DOT_CHUNK) ? static_cast<int>(n - base) : DOT_CHUNK;
     const unsigned char* a = static_cast<const unsigned char*>(A) + base * ES;
     const unsigned char* b = static_cast<const unsigned char*>(B) + base * ES;
-    pdl_launch_dependents();
     if (prefetch_first && threadIdx.x == 0) dot_prefetch(a, b, static_cast<size_t>(len) * ES, size_t{ROWS} * DOT_LANES * ES);
     pdl_wait();
 
@@ -300,7 +298,6 @@ __global__ void __launch_bounds__(DOT_FINAL_THREADS)
 dot_final(double* p, size_t k, size_t stride, double* out)
 {
     __shared__ double warp_sums[32];
-    pdl_launch_dependents();
     pdl_wait();
     const size_t j0 = static_cast<size_t>(blockIdx.x) * DOT_FINAL_BLOCK + static_cast<size_t>(threadIdx.x) * DOT_FINAL_PER_THREAD;
     double x[DOT_FINAL_PER_THREAD];

@@ -49,9 +49,11 @@ inline int current_dev_info(const b200va_devinfo_t** out)
     return dev_info(device, out);
 }
 
-// Programmatic stream serialization lets launch k+1 ramp up behind launch k's tail (the kernels
-// call griddepcontrol.wait before their first global access, so stream order is unchanged).  Every
-// hot-path launch uses it unless B200VA_NO_PDL=1.
+// Programmatic stream serialization lets launch k+1 ramp up behind launch k's tail.  The kernels call
+// griddepcontrol.wait before their first global access, except the early-load forms (vadd_vec and
+// vadd_vec_dyn with EARLY = 1), which load their first tile before it; each kernel releases its successor
+// only after its own wait (b200va_ptx.cuh: pdl_wait), so launch k is the only launch that can still be
+// running beside launch k+1.  Every hot-path launch uses it unless B200VA_NO_PDL=1.
 bool pdl_enabled();
 
 // Restores the calling thread's current device on every exit path of the entry points that

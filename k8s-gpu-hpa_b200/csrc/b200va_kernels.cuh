@@ -62,7 +62,6 @@ template <int U>
 __global__ void vadd_scalar_unrolled(const float* A, const float* B, float* C, size_t n)
 {
     const size_t base = static_cast<size_t>(blockIdx.x) * blockDim.x * U + threadIdx.x;
-    pdl_launch_dependents();
     pdl_wait();
     float a[U], b[U];
 #pragma unroll
@@ -182,7 +181,6 @@ __global__ void vadd_vec(const float* A, const float* B, float* C, size_t n, siz
     const float* b = B + head;
     float* c = C + head;
     const size_t tile_vecs = static_cast<size_t>(blockDim.x) * UNROLL;
-    pdl_launch_dependents();
     if constexpr (EARLY == 2) prefetch_first_tile<VW>(a, b, blockIdx.x, tile_vecs, nvec);
     bool waited = EARLY != 1;
     if constexpr (EARLY != 1) pdl_wait();   // everything above overlapped the previous launch's tail
@@ -212,7 +210,6 @@ __global__ void vadd_vec_dyn(const float* A, const float* B, float* C, size_t n,
     const float* b = B + head;
     float* c = C + head;
     const size_t tile_vecs = static_cast<size_t>(blockDim.x) * UNROLL;
-    pdl_launch_dependents();
     if constexpr (EARLY == 2) prefetch_first_tile<VW>(a, b, blockIdx.x, tile_vecs, nvec);
     bool waited = EARLY != 1;
     if constexpr (EARLY != 1) pdl_wait();
@@ -305,7 +302,6 @@ vadd_tma(const float* A, const float* B, float* C, size_t n, size_t head, size_t
 
     uint64_t pol = 0;
     if constexpr (L2_HINT || ST == ST_NA_EF) pol = l2_evict_first_policy();
-    pdl_launch_dependents();
     pdl_wait();   // barrier init and address math overlapped the previous launch's tail
 
     if (threadIdx.x < 32) {
@@ -409,7 +405,6 @@ vadd_tma_dyn(const float* A, const float* B, float* C, size_t n, size_t head, si
 
     uint64_t pol = 0;
     if constexpr (L2_HINT || ST == ST_NA_EF) pol = l2_evict_first_policy();
-    pdl_launch_dependents();
     pdl_wait();
 
     if (threadIdx.x < 32) {
@@ -469,7 +464,6 @@ vadd_tma_dyn(const float* A, const float* B, float* C, size_t n, size_t head, si
 // next to the add's 2:1 mix (b200va_probe_f32).
 __global__ void probe_read2(const float* A, const float* B, float* C, size_t nvec)
 {
-    pdl_launch_dependents();
     pdl_wait();
     const size_t v = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     float sum = 0.f;
@@ -482,7 +476,6 @@ __global__ void probe_read2(const float* A, const float* B, float* C, size_t nve
 
 __global__ void probe_fill(float* C, size_t nvec, float value)
 {
-    pdl_launch_dependents();
     pdl_wait();
     const size_t v = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (v < nvec) stg128<ST_NA>(C + v * 4, f32x4{value, value, value, value}, 0);
@@ -490,7 +483,6 @@ __global__ void probe_fill(float* C, size_t nvec, float value)
 
 __global__ void probe_copy(const float* A, float* C, size_t nvec)
 {
-    pdl_launch_dependents();
     pdl_wait();
     const size_t v = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (v < nvec) stg128<ST_NA>(C + v * 4, ldg128<LD_PLAIN>(A + v * 4, 0), 0);

@@ -220,20 +220,17 @@ __device__ __forceinline__ void fence_proxy_async_smem()
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// Programmatic dependent launch (sm_90+).  `pdl_launch_dependents` lets the NEXT kernel in
-// the stream start scheduling its CTAs as soon as every CTA of this grid has issued it
-// (or exited); `pdl_wait` blocks until the PREVIOUS grid has completed and its memory
-// operations are visible.  Together they hide launch latency and CTA ramp-up behind the
-// previous launch's tail without weakening stream order.  Both are no-ops for a launch
-// without the programmatic-stream-serialization attribute.
-__device__ __forceinline__ void pdl_launch_dependents()
-{
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-
+// Programmatic dependent launch (sm_90+).  `pdl_wait` blocks until the PREVIOUS grid has completed
+// and its memory operations are visible, and then lets the NEXT kernel in the stream start
+// scheduling its CTAs once every CTA of this grid has done the same (or exited).  This hides
+// launch latency and CTA ramp-up behind the previous launch's tail.  The release comes only after
+// the wait, so when a kernel starts, every launch before the one immediately preceding it has
+// completed: an early-load kernel (vadd_vec EARLY = 1) can overlap that one launch and no older
+// one.  A no-op for a launch without the programmatic-stream-serialization attribute.
 __device__ __forceinline__ void pdl_wait()
 {
     asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- dynamic tile scheduler

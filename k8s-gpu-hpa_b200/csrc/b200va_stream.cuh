@@ -150,7 +150,6 @@ __global__ void stream_vec(const void* A, const void* B, void* C, size_t n, size
     const unsigned char* b = static_cast<const unsigned char*>(B) + head * ES;
     unsigned char* c = static_cast<unsigned char*>(C) + head * ES;
     const size_t tile_vecs = static_cast<size_t>(blockDim.x) * UNROLL;
-    pdl_launch_dependents();
     if (prefetch_first && threadIdx.x == 0 && blockIdx.x * tile_vecs < nvec) {
         const size_t t0 = blockIdx.x * tile_vecs;
         const uint32_t bytes = static_cast<uint32_t>((nvec - t0 < tile_vecs ? nvec - t0 : tile_vecs) * 16);

@@ -183,7 +183,7 @@ def _sass(fn: str) -> str:
     return subprocess.run(["cuobjdump", "-sass", "-fun", fn, capi.LIB_PATH], capture_output=True, text=True).stdout
 
 
-def test_convert_kernels_in_the_sass():
+def test_convert_kernels_in_the_sass_wait_before_they_release_the_next_launch():
     sass = subprocess.run(["cuobjdump", "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
     names = sorted(set(re.findall(r"Function : (_ZN6b200va\d+convert_\w+)", sass)))
     assert len(names) == 12, names
@@ -192,7 +192,7 @@ def test_convert_kernels_in_the_sass():
         body = _sass(fn)
         src, dst = (k for c in re.search(r"ILi(\d)ELi(\d)E", fn).groups() for k, v in code.items() if v == int(c))
         ops = re.findall(r"\b(LDG\.E\S*|STG\.E\S*|ACQBULK|UBLKPF\.L2|PREEXIT)\b", body)
-        assert ops[:3] == ["PREEXIT", "UBLKPF.L2", "ACQBULK"], (fn, ops[:4])
+        assert ops[:2] == ["UBLKPF.L2", "ACQBULK"] and "PREEXIT" in ops[2:], (fn, ops[:4])   # the trigger after the wait
         assert "LDG.E.128" in ops and any(re.fullmatch(r"STG\.E\S*\.128", o) for o in ops), fn
         if src == "f64" and dst in ("f16", "bf16"):
             want = "F2F.F16.F64" if dst == "f16" else "F2F.BF16.F64"

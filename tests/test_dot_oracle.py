@@ -214,9 +214,9 @@ def _sass(fn: str) -> list[str]:
     return re.findall(r"\b(LDG\.E\S*|LDS\S*|STG\.E\S*|ACQBULK|UBLKPF\.L2|PREEXIT)\b", out)
 
 
-def test_dot_kernels_load_nothing_before_the_dependency_wait():
-    """The trigger (PREEXIT) comes first; before griddepcontrol.wait (ACQBULK) only the two L2 prefetches of the
-    HBM class; every global load and store after it."""
+def test_dot_kernels_load_nothing_and_release_nothing_before_the_dependency_wait():
+    """Before griddepcontrol.wait (ACQBULK) only the two L2 prefetches of the HBM class; the trigger (PREEXIT) and
+    every global load and store after it."""
     sass = subprocess.run(["cuobjdump", "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
     names = sorted(set(re.findall(r"Function : (_ZN6b200va\d+dot_\w+)", sass)))
     assert len(names) == 9, names                    # dot_vec and dot_scalar per type, dot_final
@@ -224,9 +224,9 @@ def test_dot_kernels_load_nothing_before_the_dependency_wait():
         ops = _sass(fn)
         assert "ACQBULK" in ops, fn
         before = ops[:ops.index("ACQBULK")]
-        assert before[0] == "PREEXIT", (fn, before)
         want = [] if "dot_final" in fn else ["UBLKPF.L2", "UBLKPF.L2"]
-        assert before[1:] == want, (fn, before)
+        assert before == want, (fn, before)
+        assert "PREEXIT" in ops[ops.index("ACQBULK"):], fn
         assert any(o.startswith("LDG") for o in ops[ops.index("ACQBULK"):]), fn
     vec = [fn for fn in names if "dot_vec" in fn]
     assert len(vec) == 4 and all(any(o.startswith("LDG.E.128") for o in _sass(fn)) for fn in vec)
