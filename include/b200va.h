@@ -290,6 +290,31 @@ int b200va_stream(int op, int dtype, const void *dA, const void *dB, void *dC, s
  * capturable in a CUDA graph. */
 int b200va_convert(int src_dtype, const void *dA, int dst_dtype, void *dC, size_t n, void *stream);
 
+/* ---- FP8 quantize and dequantize (row f4) ---------------------------------------------------
+ * The two OCP FP8 formats of the H100's FP8 tensor cores, one byte per element: */
+#define B200VA_F8_E4M3 0   /* OCP FP8 E4M3 ("e4m3fn"): bias 7, no infinities, max finite 448, NaN = S.1111.111 */
+#define B200VA_F8_E5M2 1   /* OCP FP8 E5M2: bias 15, IEEE-style +-inf and NaNs, max finite 57344 */
+/* Quantize: c[i] = sat(RN(a[i] * 2^scale_exp)), src_dtype a B200VA_DT_* code.  The product is exact and is
+ * rounded once to the FP8 format (round-to-nearest-even, the format's subnormals, no FTZ on either side).  A
+ * magnitude above the largest finite value -- values that round past it and +-inf included -- gives +-max finite
+ * (448 or 57344: the hardware's .satfinite); a NaN gives a NaN; +-0 and values that round to zero keep their sign.
+ * d_amax (may be NULL) max-accumulates the largest unscaled magnitude: *d_amax = max(*d_amax, max_i |a_i|), the a_i
+ * widened exactly to f64, a NaN anywhere making it a NaN.  Set *d_amax to +0.0 before the first call; shards and
+ * repeated calls then combine.  The max is exact, so the result does not depend on the order of reduction.
+ * Dequantize: c[i] = a[i] * 2^-scale_exp rounded once to dst_dtype by b200va_convert's rules (RNE, no FTZ,
+ * overflow to +-inf); E5M2 +-inf stays +-inf, a NaN gives a NaN.  Dequantizing with the scale_exp a tensor was
+ * quantized with gives its FP8 values scaled back, exactly whenever the destination can hold them.
+ * scale_exp must lie in [-126, 126].
+ * B200VA_ERR_VARIANT: bad dtype or FP8 code.  B200VA_ERR_INVALID: scale_exp out of range, NULL dA/dC with n > 0,
+ * n > 2^40.  B200VA_ERR_ALIGN: dA/dC not aligned to their element size, d_amax not 8-byte aligned.
+ * B200VA_ERR_OVERLAP: C meets A anywhere, or d_amax meets A or C.  n = 0 writes nothing.
+ * Asynchronous on `stream`: one kernel launch, no allocation, synchronisation or memset; capturable in a CUDA
+ * graph.  The d_amax update is one atomic per CTA. */
+int b200va_quantize_fp8(int src_dtype, const void *dA, int fp8, void *dC, size_t n,
+                        int scale_exp, double *d_amax, void *stream);
+int b200va_dequantize_fp8(int fp8, const void *dA, int dst_dtype, void *dC, size_t n,
+                          int scale_exp, void *stream);
+
 /* ---- reproducible dot product (row f4) --------------------------------------------------
  * *d_out = sum_i a_i b_i as a binary64 value in device memory, written asynchronously on `stream`
  * (not rounded to the storage type; dtype is a B200VA_DT_* code).  Every operand is widened

@@ -28,6 +28,8 @@ STAGE_AUTO, STAGE_SLOTS, STAGE_ZEROCOPY, STAGE_LANES, STAGE_BOUNCE, STAGE_REGIST
 PROBES = {"read2": 0, "fill": 1, "copy": 2}
 OPS = {"copy": 0, "scale": 1, "add": 2, "triad": 3}
 DTYPES = {"f32": 0, "f64": 1, "f16": 2, "bf16": 3}
+F8_E4M3, F8_E5M2 = 0, 1                    # b200va_quantize_fp8 / b200va_dequantize_fp8 formats (B200VA_F8_*)
+F8 = {"e4m3": F8_E4M3, "e5m2": F8_E5M2}
 DOT_LANES, DOT_CHUNK = 2048, 65536         # b200va_dot's lane count and chunk size (B200VA_DOT_*)
 VARIANTS = {"auto": K_AUTO, "k0": K0_SCALAR, "k1": K1_VEC128, "k2": K2_TMA, "k3": K3_VEC256}
 
@@ -109,6 +111,8 @@ _SIGS = {
     "b200va_device_numa_node_of": (_I, [_I]),
     "b200va_stream": (_I, [_I, _I, _P, _P, _P, _SZ, C.c_double, _P]),
     "b200va_convert": (_I, [_I, _P, _I, _P, _SZ, _P]),
+    "b200va_quantize_fp8": (_I, [_I, _P, _I, _P, _SZ, _I, _P, _P]),
+    "b200va_dequantize_fp8": (_I, [_I, _P, _I, _P, _SZ, _I, _P]),
     "b200va_dot_workspace_bytes": (_SZ, [_SZ]),
     "b200va_dot": (_I, [_I, _P, _P, _SZ, _P, _P, _SZ, _P]),
     "b200va_probe_f32": (_I, [_I, _P, _P, _P, _SZ, _P]),

@@ -1,8 +1,9 @@
-// b200va_typed.cu -- the STREAM ops (copy, scale, add, triad), the reproducible dot product and the
-// conversions between f32, f64, f16 and bf16.  The only unit that includes the STREAM, dot and convert
-// kernels (b200va_dot.cuh and b200va_convert.cuh, which include b200va_stream.cuh).
+// b200va_typed.cu -- the STREAM ops (copy, scale, add, triad), the reproducible dot product, the
+// conversions between f32, f64, f16 and bf16, and the FP8 quantize and dequantize.  The only unit that
+// includes the STREAM, dot, convert and FP8 kernels (b200va_dot.cuh and b200va_fp8.cuh, which include
+// b200va_convert.cuh and b200va_stream.cuh).
 #include "b200va_internal.h"
-#include "b200va_convert.cuh"
+#include "b200va_fp8.cuh"
 #include "b200va_dot.cuh"
 
 using namespace b200va;
@@ -131,6 +132,53 @@ int launch_convert_typed(const void* dA, void* dC, size_t n, cudaStream_t st)
                          prefetch_first);
 }
 
+// b200va_quantize_fp8 (QUANT: T -> fmt) and b200va_dequantize_fp8 (fmt -> T): one fp8_quant_vec<T> or
+// fp8_dequant_vec<T> launch, the format passed to the kernel; planned as convert_vec's with G = 16.  The head is
+// the smallest h < 16 at which A and C both sit on a 16-byte boundary (head = n in mixed phase).  A thread's unit of work is a group of 16 when quantizing and a
+// 16-byte output slice (sizeof T per group) when dequantizing.  The geometry follows the HBM class of the wider
+// operand (T), as convert's does: 512 x 2 with the L2 prefetch there, 256 x 1 below it.
+template <bool QUANT, int T>
+int launch_fp8_typed(const void* dA, void* dC, size_t n, int fmt, int k, double* amax, cudaStream_t st)
+{
+    constexpr size_t ES = dt_traits<T>::size, ESA = QUANT ? ES : 1, ESC = QUANT ? 1 : ES;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC);
+    size_t head = n;
+    for (size_t h = head_peel(a, ESA); h < 16; h += 16 / ESA)
+        if (((c + h * ESC) & 15u) == 0) { head = h; break; }
+    if (head > n) head = n;
+    const size_t ngroups = (n - head) / 16;
+    const size_t units = QUANT ? ngroups : ngroups * ES;
+    const size_t edges = n - ngroups * 16;
+    const bool hbm = hbm_class(n, ES);
+    const unsigned threads = hbm ? 512 : 256;
+    const int unroll = hbm ? 2 : 1;
+    const int prefetch_first = hbm ? 1 : 0;
+    const size_t tile = static_cast<size_t>(threads) * unroll;
+    const size_t blocks = std::max((units + tile - 1) / tile, (edges + threads - 1) / threads);
+    const unsigned grid = static_cast<unsigned>(std::max<size_t>(std::min<size_t>(blocks, 0x7fffffff), 1));
+    if constexpr (QUANT)
+        return launch_kernel(fp8_quant_vec<T>, grid, threads, 0, st, pdl_enabled(), dA, dC, n, head, ngroups, unroll,
+                             prefetch_first, fmt, k, amax);
+    else
+        return launch_kernel(fp8_dequant_vec<T>, grid, threads, 0, st, pdl_enabled(), dA, dC, n, head, ngroups, unroll,
+                             prefetch_first, fmt, k);
+}
+
+// The argument rules the two FP8 entry points share, after the dtype and format codes: scale_exp in [-126, 126],
+// then A and C as b200va_convert checks them (1-byte FP8 elements), then d_amax (may be NULL) 8-byte aligned and
+// meeting neither A nor C.
+int check_fp8_args(size_t es, const void* dA, size_t esc, const void* dC, size_t n, int k, const double* d_amax)
+{
+    if (k < -126 || k > 126) return B200VA_ERR_INVALID;
+    RC_TRY(check_convert_operands(es, dA, esc, dC, n));
+    const uintptr_t m = reinterpret_cast<uintptr_t>(d_amax), a = reinterpret_cast<uintptr_t>(dA),
+                    c = reinterpret_cast<uintptr_t>(dC);
+    if (m & 7u) return B200VA_ERR_ALIGN;
+    auto meet = [&](uintptr_t x, size_t bytes) { return m && n && m < x + bytes && x < m + 8; };
+    if (meet(a, n * es) || meet(c, n * esc)) return B200VA_ERR_OVERLAP;
+    return B200VA_OK;
+}
+
 }  // namespace
 
 // ========================================= ABI (C linkage from the declarations in include/b200va.h)
@@ -162,6 +210,33 @@ int b200va_convert(int src_dtype, const void* dA, int dst_dtype, void* dC, size_
         with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dst_dtype, [&](auto DST) {
             if constexpr (SRC != DST) rc = launch_convert_typed<SRC, DST>(dA, dC, n, st);
         });
+    });
+    return rc;
+}
+
+int b200va_quantize_fp8(int src_dtype, const void* dA, int fp8, void* dC, size_t n, int scale_exp, double* d_amax,
+                        void* stream)
+{
+    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    RC_TRY(check_fp8_args(dtype_size(src_dtype), dA, 1, dC, n, scale_exp, d_amax));
+    if (n == 0) return B200VA_OK;
+    int rc = B200VA_ERR_VARIANT;
+    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(src_dtype, [&](auto SRC) {
+        rc = launch_fp8_typed<true, SRC>(dA, dC, n, fp8, scale_exp, d_amax, static_cast<cudaStream_t>(stream));
+    });
+    return rc;
+}
+
+int b200va_dequantize_fp8(int fp8, const void* dA, int dst_dtype, void* dC, size_t n, int scale_exp, void* stream)
+{
+    if (dst_dtype < 0 || dst_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    RC_TRY(check_fp8_args(1, dA, dtype_size(dst_dtype), dC, n, scale_exp, nullptr));
+    if (n == 0) return B200VA_OK;
+    int rc = B200VA_ERR_VARIANT;
+    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dst_dtype, [&](auto DST) {
+        rc = launch_fp8_typed<false, DST>(dA, dC, n, fp8, scale_exp, nullptr, static_cast<cudaStream_t>(stream));
     });
     return rc;
 }

@@ -161,6 +161,76 @@ def convert(a, dtype, out=None, *, stream=None):
     return out
 
 
+def _fp8_format(fmt):
+    """(torch dtype, B200VA_F8_* code) of an FP8 format given as a torch dtype or "e4m3" / "e5m2"."""
+    torch = _torch()
+    dtypes = {"e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
+    if isinstance(fmt, str):
+        if fmt not in dtypes:
+            raise TypeError(f"fmt must be one of {sorted(dtypes)}, got {fmt!r}")
+        fmt = dtypes[fmt]
+    codes = {v: capi.F8[k] for k, v in dtypes.items()}
+    if fmt not in codes:
+        raise TypeError(f"fmt must be torch.float8_e4m3fn or torch.float8_e5m2, got {fmt}")
+    return fmt, codes[fmt]
+
+
+def _fp8_out(out, dtype, a):
+    torch = _torch()
+    if out is None:
+        return torch.empty(a.shape, dtype=dtype, device=a.device)
+    if (not isinstance(out, torch.Tensor) or out.dtype != dtype or out.numel() != a.numel() or out.device != a.device
+            or not out.is_contiguous()):
+        raise TypeError("out must be a contiguous tensor of the result dtype with a's length on a's device")
+    return out
+
+
+def quantize_fp8(a, fmt, *, scale_exp: int = 0, amax=None, out=None, stream=None):
+    """``a`` (f32/f64/f16/bf16) times 2^scale_exp, rounded once to FP8 (b200va_quantize_fp8): round-to-nearest-even,
+    saturating at +-max finite (448 for E4M3, 57344 for E5M2), inf included; NaN stays NaN.  ``fmt``:
+    torch.float8_e4m3fn / torch.float8_e5m2 or "e4m3" / "e5m2".  ``amax``: a one-element float64 CUDA tensor that
+    max-accumulates max |a| (unscaled; NaN if any element is); set it to 0 before the first call.  ``out``: a
+    contiguous CUDA tensor of the FP8 dtype with a's length on a's device, else a new one.  Asynchronous on the
+    current stream."""
+    torch = _torch()
+    names = {getattr(torch, v): k for k, v in _TORCH_DT.items()}
+    if not isinstance(a, torch.Tensor) or not a.is_cuda or a.dtype not in names or not a.is_contiguous():
+        raise TypeError("a must be a contiguous CUDA tensor of float32/float64/float16/bfloat16")
+    dtype, code = _fp8_format(fmt)
+    out = _fp8_out(out, dtype, a)
+    if amax is not None and (not isinstance(amax, torch.Tensor) or amax.dtype != torch.float64 or amax.numel() != 1
+                             or amax.device != a.device):
+        raise TypeError("amax must be a one-element float64 tensor on a's device")
+    with torch.cuda.device(a.device):
+        check(lib.b200va_quantize_fp8(capi.DTYPES[names[a.dtype]], a.data_ptr(), code, out.data_ptr(), a.numel(),
+                                      int(scale_exp), amax.data_ptr() if amax is not None else None, _stream_ptr(stream)),
+              "b200va_quantize_fp8")
+    return out
+
+
+def dequantize_fp8(a, dtype, *, scale_exp: int = 0, out=None, stream=None):
+    """FP8 ``a`` (torch.float8_e4m3fn / float8_e5m2) times 2^-scale_exp, rounded once to ``dtype``
+    (torch.float32/float64/float16/bfloat16, or "f32"/"f64"/"f16"/"bf16") by b200va_dequantize_fp8: round-to-nearest-
+    even, no FTZ, overflow to inf.  ``out``: a contiguous CUDA tensor of ``dtype`` with a's length on a's device, else
+    a new one.  Asynchronous on the current stream."""
+    torch = _torch()
+    names = {getattr(torch, v): k for k, v in _TORCH_DT.items()}
+    if not isinstance(a, torch.Tensor) or not a.is_cuda or not a.is_contiguous():
+        raise TypeError("a must be a contiguous CUDA tensor of float8_e4m3fn/float8_e5m2")
+    _, code = _fp8_format(a.dtype)
+    if isinstance(dtype, str):
+        if dtype not in _TORCH_DT:
+            raise TypeError(f"dtype must be one of {sorted(_TORCH_DT)}, got {dtype!r}")
+        dtype = getattr(torch, _TORCH_DT[dtype])
+    if dtype not in names:
+        raise TypeError(f"dtype must be float32/float64/float16/bfloat16, got {dtype}")
+    out = _fp8_out(out, dtype, a)
+    with torch.cuda.device(a.device):
+        check(lib.b200va_dequantize_fp8(code, a.data_ptr(), capi.DTYPES[names[dtype]], out.data_ptr(), a.numel(),
+                                        int(scale_exp), _stream_ptr(stream)), "b200va_dequantize_fp8")
+    return out
+
+
 def dot(a, b, *, out=None, workspace=None, stream=None):
     """The reproducible dot product of two equal-length contiguous CUDA tensors of one of f32/f64/f16/bf16
     (b200va_dot): a 0-d float64 CUDA tensor, written asynchronously on the current stream.  The bits
