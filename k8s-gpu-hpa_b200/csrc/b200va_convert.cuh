@@ -80,16 +80,115 @@ __device__ __forceinline__ void convert_words(const uint32_t* s, uint32_t* d)
     }
 }
 
+// ---- the pieces every cast kernel shares -------------------------------------------------------------
+// The BYTES (1, 2, 4 or 8) bytes at p, BYTES-aligned, zero-extended; and the low BYTES bytes of v stored to p.
+template <int BYTES>
+__device__ __forceinline__ unsigned long long ld_bits(const unsigned char* p)
+{
+    if constexpr (BYTES == 8) return *reinterpret_cast<const unsigned long long*>(p);
+    else if constexpr (BYTES == 4) return *reinterpret_cast<const uint32_t*>(p);
+    else if constexpr (BYTES == 2) return *reinterpret_cast<const unsigned short*>(p);
+    else return *p;
+}
+
+template <int BYTES>
+__device__ __forceinline__ void st_bits(unsigned char* p, unsigned long long v)
+{
+    if constexpr (BYTES == 8) *reinterpret_cast<unsigned long long*>(p) = v;
+    else if constexpr (BYTES == 4) *reinterpret_cast<uint32_t*>(p) = static_cast<uint32_t>(v);
+    else if constexpr (BYTES == 2) *reinterpret_cast<unsigned short*>(p) = static_cast<unsigned short>(v);
+    else *p = static_cast<unsigned char>(v);
+}
+
+// V consecutive 16-byte vectors, as a value a tile can hold per unit.
+template <int V>
+struct vecs { u32x4 v[V]; };
+
+// Unit u of a body of V-vector units at p.
+template <int V>
+__device__ __forceinline__ vecs<V> ld_vecs(const unsigned char* p, size_t u)
+{
+    vecs<V> r;
+#pragma unroll
+    for (int k = 0; k < V; ++k) r.v[k] = ldg128_bits<LD_PLAIN>(p + (u * V + k) * 16);
+    return r;
+}
+
+// The 32-bit words of V vectors, in memory order.
+template <int V>
+__device__ __forceinline__ void unpack(const u32x4* v, uint32_t* w)
+{
+#pragma unroll
+    for (int k = 0; k < V; ++k) {
+        w[4 * k] = v[k].x; w[4 * k + 1] = v[k].y; w[4 * k + 2] = v[k].z; w[4 * k + 3] = v[k].w;
+    }
+}
+
+// With prefetch_first, thread 0 bulk-prefetches the CTA's first tile of A into L2 (units of PER_UNIT elements of
+// ES bytes, from element head on) ahead of the programmatic dependency: always legal, L2 is the point of coherence.
+template <int PER_UNIT, int ES>
+__device__ __forceinline__ void prefetch_first_tile(int prefetch_first, const unsigned char* a, size_t head, size_t nunits,
+                                                    int unroll)
+{
+    if (prefetch_first && threadIdx.x == 0) {
+        const size_t tile = static_cast<size_t>(blockDim.x) * unroll, u0 = blockIdx.x * tile;
+        if (u0 < nunits)
+            bulk_prefetch_l2(a + (head + u0 * PER_UNIT) * ES,
+                             static_cast<uint32_t>((nunits - u0 < tile ? nunits - u0 : tile) * PER_UNIT * ES));
+    }
+}
+
+// The vector body: tiles of blockDim.x * U units, grid-strided; thread t takes units t + j blockDim.x of a tile.
+// load(u) reads unit u and put(u, x) computes and stores it.  A full tile issues all U loads before its first store;
+// a partial tile guards each unit.
+template <int U, class Load, class Put>
+__device__ __forceinline__ void cast_tiles(size_t nunits, Load load, Put put)
+{
+    const size_t tile = static_cast<size_t>(blockDim.x) * U;
+    for (size_t t = blockIdx.x; t * tile < nunits; t += gridDim.x) {
+        const size_t u0 = t * tile + threadIdx.x;
+        if ((t + 1) * tile <= nunits) {
+            decltype(load(u0)) in[U];
+#pragma unroll
+            for (int j = 0; j < U; ++j) in[j] = load(u0 + static_cast<size_t>(j) * blockDim.x);
+#pragma unroll
+            for (int j = 0; j < U; ++j) put(u0 + static_cast<size_t>(j) * blockDim.x, in[j]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < U; ++j) {
+                const size_t u = u0 + static_cast<size_t>(j) * blockDim.x;
+                if (u < nunits) put(u, load(u));
+            }
+        }
+    }
+}
+
+// The launch's unroll (1 or 2) to cast_tiles.
+template <class Load, class Put>
+__device__ __forceinline__ void cast_tiles(int unroll, size_t nunits, Load load, Put put)
+{
+    if (unroll == 2) cast_tiles<2>(nunits, load, put);
+    else cast_tiles<1>(nunits, load, put);
+}
+
+// The elements outside the vector body [head, body_end) -- the head and the tail, or all n in mixed phase (head = n)
+// -- grid-strided, elem(e) for each.
+template <class Elem>
+__device__ __forceinline__ void cast_edges(size_t n, size_t head, size_t body_end, Elem elem)
+{
+    const size_t edges = head + (n - body_end);
+    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < edges; i += stride)
+        elem(i < head ? i : body_end + (i - head));
+}
+
 // One group: VS source vectors in, VD destination vectors out.
 template <int SRC, int DST>
 __device__ __forceinline__ void convert_group(const u32x4* in, u32x4* out)
 {
     using S = convert_shape<SRC, DST>;
     uint32_t s[4 * S::VS], d[4 * S::VD];
-#pragma unroll
-    for (int k = 0; k < S::VS; ++k) {
-        s[4 * k] = in[k].x; s[4 * k + 1] = in[k].y; s[4 * k + 2] = in[k].z; s[4 * k + 3] = in[k].w;
-    }
+    unpack<S::VS>(in, s);
     convert_words<SRC, DST, S::G>(s, d);
 #pragma unroll
     for (int k = 0; k < S::VD; ++k) out[k] = u32x4{d[4 * k], d[4 * k + 1], d[4 * k + 2], d[4 * k + 3]};
@@ -100,93 +199,34 @@ template <int SRC, int DST>
 __device__ __forceinline__ void convert_elem(const unsigned char* a, unsigned char* c)
 {
     using S = convert_shape<SRC, DST>;
-    uint32_t s[2] = {0, 0}, d[2];
-    if constexpr (S::ESS == 8) {
-        const unsigned long long x = *reinterpret_cast<const unsigned long long*>(a);
-        s[0] = static_cast<uint32_t>(x);
-        s[1] = static_cast<uint32_t>(x >> 32);
-    } else if constexpr (S::ESS == 4) {
-        s[0] = *reinterpret_cast<const uint32_t*>(a);
-    } else {
-        s[0] = *reinterpret_cast<const unsigned short*>(a);
-    }
+    const unsigned long long x = ld_bits<S::ESS>(a);
+    const uint32_t s[2] = {static_cast<uint32_t>(x), static_cast<uint32_t>(x >> 32)};
+    uint32_t d[2] = {0, 0};
     convert_words<SRC, DST, 1>(s, d);
-    if constexpr (S::ESD == 8) *reinterpret_cast<unsigned long long*>(c) = d[0] | (static_cast<unsigned long long>(d[1]) << 32);
-    else if constexpr (S::ESD == 4) *reinterpret_cast<uint32_t*>(c) = d[0];
-    else *reinterpret_cast<unsigned short*>(c) = static_cast<unsigned short>(d[0]);
-}
-
-// ---- the vector body --------------------------------------------------------------------------------
-// Tiles of blockDim.x * U groups, grid-strided; thread t takes groups t + j blockDim.x of a tile.  A full
-// tile issues all U * VS loads before its first store.
-template <int SRC, int DST, int U>
-__device__ __forceinline__ void convert_tiles(const unsigned char* a, unsigned char* c, size_t ngroups)
-{
-    using S = convert_shape<SRC, DST>;
-    const size_t tile = static_cast<size_t>(blockDim.x) * U;
-    for (size_t t = blockIdx.x; t * tile < ngroups; t += gridDim.x) {
-        const size_t g0 = t * tile + threadIdx.x;
-        if ((t + 1) * tile <= ngroups) {
-            u32x4 in[U][S::VS];
-#pragma unroll
-            for (int j = 0; j < U; ++j)
-#pragma unroll
-                for (int k = 0; k < S::VS; ++k)
-                    in[j][k] = ldg128_bits<LD_PLAIN>(a + ((g0 + static_cast<size_t>(j) * blockDim.x) * S::VS + k) * 16);
-#pragma unroll
-            for (int j = 0; j < U; ++j) {
-                u32x4 out[S::VD];
-                convert_group<SRC, DST>(in[j], out);
-#pragma unroll
-                for (int k = 0; k < S::VD; ++k)
-                    stg128_bits<ST_NA>(c + ((g0 + static_cast<size_t>(j) * blockDim.x) * S::VD + k) * 16, out[k]);
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < U; ++j) {
-                const size_t g = g0 + static_cast<size_t>(j) * blockDim.x;
-                if (g < ngroups) {
-                    u32x4 in[S::VS], out[S::VD];
-#pragma unroll
-                    for (int k = 0; k < S::VS; ++k) in[k] = ldg128_bits<LD_PLAIN>(a + (g * S::VS + k) * 16);
-                    convert_group<SRC, DST>(in, out);
-#pragma unroll
-                    for (int k = 0; k < S::VD; ++k) stg128_bits<ST_NA>(c + (g * S::VD + k) * 16, out[k]);
-                }
-            }
-        }
-    }
+    st_bits<S::ESD>(c, d[0] | static_cast<unsigned long long>(d[1]) << 32);
 }
 
 // ---- the kernel -------------------------------------------------------------------------------------
-// Elements [head, head + G ngroups) are the vector body, at 16-byte boundaries in A and in C; the others
-// (the head, the tail, or all n when A and C have no common boundary and the dispatcher passes head = n)
-// go through a grid-stride scalar loop.  unroll (1 or 2) and prefetch_first are the launch's geometry:
-// with prefetch_first, thread 0 bulk-prefetches the CTA's first A tile into L2 ahead of the programmatic
-// dependency (always legal: L2 is the point of coherence).
+// Elements [head, head + G ngroups) are the vector body, one group per unit, at 16-byte boundaries in A and in C;
+// the others go through cast_edges.  unroll (1 or 2) and prefetch_first are the launch's geometry.
 template <int SRC, int DST>
 __global__ void convert_vec(const void* A, void* C, size_t n, size_t head, size_t ngroups, int unroll, int prefetch_first)
 {
     using S = convert_shape<SRC, DST>;
     const unsigned char* a = static_cast<const unsigned char*>(A);
     unsigned char* c = static_cast<unsigned char*>(C);
-    if (prefetch_first && threadIdx.x == 0) {
-        const size_t tile = static_cast<size_t>(blockDim.x) * unroll, g0 = blockIdx.x * tile;
-        if (g0 < ngroups)
-            bulk_prefetch_l2(a + (head + g0 * S::G) * S::ESS,
-                             static_cast<uint32_t>((ngroups - g0 < tile ? ngroups - g0 : tile) * S::G * S::ESS));
-    }
+    prefetch_first_tile<S::G, S::ESS>(prefetch_first, a, head, ngroups, unroll);
     pdl_wait();
 
-    if (unroll == 2) convert_tiles<SRC, DST, 2>(a + head * S::ESS, c + head * S::ESD, ngroups);
-    else convert_tiles<SRC, DST, 1>(a + head * S::ESS, c + head * S::ESD, ngroups);
-
-    const size_t body_end = head + ngroups * S::G, edges = head + (n - body_end);
-    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < edges; i += stride) {
-        const size_t e = i < head ? i : body_end + (i - head);
-        convert_elem<SRC, DST>(a + e * S::ESS, c + e * S::ESD);
-    }
+    const unsigned char* ab = a + head * S::ESS;
+    unsigned char* cb = c + head * S::ESD;
+    cast_tiles(unroll, ngroups, [=](size_t g) { return ld_vecs<S::VS>(ab, g); }, [=](size_t g, const vecs<S::VS>& in) {
+        u32x4 out[S::VD];
+        convert_group<SRC, DST>(in.v, out);
+#pragma unroll
+        for (int k = 0; k < S::VD; ++k) stg128_bits<ST_NA>(cb + (g * S::VD + k) * 16, out[k]);
+    });
+    cast_edges(n, head, head + ngroups * S::G, [=](size_t e) { convert_elem<SRC, DST>(a + e * S::ESS, c + e * S::ESD); });
 }
 
 }  // namespace b200va

@@ -89,50 +89,6 @@ __device__ __forceinline__ uint32_t quant_pair(const uint32_t* s, int e0, int k,
     return f8x2_from_f32<F8>(q[0], q[1]);
 }
 
-// Tiles of blockDim.x * U groups, grid-strided, as convert_tiles: a full tile issues all U * ESS loads first.
-template <int SRC, int F8, int U>
-__device__ __forceinline__ void quant_tiles(const unsigned char* a, unsigned char* c, size_t ngroups, int k,
-                                            amax_bits_t<SRC>& m)
-{
-    constexpr int VS = dt_traits<SRC>::size;      // 16-byte source vectors per group of 16
-    const size_t tile = static_cast<size_t>(blockDim.x) * U;
-    auto group = [&](const u32x4* in, size_t g) {
-        uint32_t s[4 * VS], d[4];
-#pragma unroll
-        for (int v = 0; v < VS; ++v) {
-            s[4 * v] = in[v].x; s[4 * v + 1] = in[v].y; s[4 * v + 2] = in[v].z; s[4 * v + 3] = in[v].w;
-        }
-#pragma unroll
-        for (int w = 0; w < 4; ++w)
-            d[w] = quant_pair<SRC, F8>(s, 4 * w, k, m) | (quant_pair<SRC, F8>(s, 4 * w + 2, k, m) << 16);
-        stg128_bits<ST_NA>(c + g * 16, u32x4{d[0], d[1], d[2], d[3]});
-    };
-    for (size_t t = blockIdx.x; t * tile < ngroups; t += gridDim.x) {
-        const size_t g0 = t * tile + threadIdx.x;
-        if ((t + 1) * tile <= ngroups) {
-            u32x4 in[U][VS];
-#pragma unroll
-            for (int j = 0; j < U; ++j)
-#pragma unroll
-                for (int v = 0; v < VS; ++v)
-                    in[j][v] = ldg128_bits<LD_PLAIN>(a + ((g0 + static_cast<size_t>(j) * blockDim.x) * VS + v) * 16);
-#pragma unroll
-            for (int j = 0; j < U; ++j) group(in[j], g0 + static_cast<size_t>(j) * blockDim.x);
-        } else {
-#pragma unroll
-            for (int j = 0; j < U; ++j) {
-                const size_t g = g0 + static_cast<size_t>(j) * blockDim.x;
-                if (g < ngroups) {
-                    u32x4 in[VS];
-#pragma unroll
-                    for (int v = 0; v < VS; ++v) in[v] = ldg128_bits<LD_PLAIN>(a + (g * VS + v) * 16);
-                    group(in, g);
-                }
-            }
-        }
-    }
-}
-
 template <class T>
 __device__ __forceinline__ T warp_max(T v)
 {
@@ -141,33 +97,28 @@ __device__ __forceinline__ T warp_max(T v)
     return v;
 }
 
-// Quantize's body after the dependency wait: elements [head, head + 16 ngroups) are the vector body, on 16-byte
-// boundaries in A and in C; the head, the tail or (mixed phase, head = n) every element go through a grid-stride
-// scalar loop.
+// Quantize's body after the dependency wait: elements [head, head + 16 ngroups) are the vector body, one group of 16
+// per unit, on 16-byte boundaries in A and in C; the others go through cast_edges.
 template <int SRC, int F8>
 __device__ __forceinline__ void quant_body(const unsigned char* a, unsigned char* c, size_t n, size_t head,
                                            size_t ngroups, int unroll, int k, amax_bits_t<SRC>& m)
 {
-    constexpr int ES = dt_traits<SRC>::size;
-    if (unroll == 2) quant_tiles<SRC, F8, 2>(a + head * ES, c + head, ngroups, k, m);
-    else quant_tiles<SRC, F8, 1>(a + head * ES, c + head, ngroups, k, m);
-
-    const size_t body_end = head + ngroups * 16, edges = head + (n - body_end);
-    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < edges; i += stride) {
-        const size_t e = i < head ? i : body_end + (i - head);
-        uint32_t s[2] = {0, 0};
-        if constexpr (ES == 8) {
-            const unsigned long long x = *reinterpret_cast<const unsigned long long*>(a + e * 8);
-            s[0] = static_cast<uint32_t>(x);
-            s[1] = static_cast<uint32_t>(x >> 32);
-        } else if constexpr (ES == 4) {
-            s[0] = *reinterpret_cast<const uint32_t*>(a + e * 4);
-        } else {
-            s[0] = *reinterpret_cast<const unsigned short*>(a + e * 2);
-        }
-        c[e] = static_cast<unsigned char>(quant_pair<SRC, F8, true>(s, 0, k, m));
-    }
+    constexpr int ES = dt_traits<SRC>::size;      // also the 16-byte source vectors per group
+    const unsigned char* ab = a + head * ES;
+    unsigned char* cb = c + head;
+    cast_tiles(unroll, ngroups, [=](size_t g) { return ld_vecs<ES>(ab, g); }, [&](size_t g, const vecs<ES>& in) {
+        uint32_t s[4 * ES], d[4];
+        unpack<ES>(in.v, s);
+#pragma unroll
+        for (int w = 0; w < 4; ++w)
+            d[w] = quant_pair<SRC, F8>(s, 4 * w, k, m) | (quant_pair<SRC, F8>(s, 4 * w + 2, k, m) << 16);
+        stg128_bits<ST_NA>(cb + g * 16, u32x4{d[0], d[1], d[2], d[3]});
+    });
+    cast_edges(n, head, head + ngroups * 16, [&](size_t e) {
+        const unsigned long long x = ld_bits<ES>(a + e * ES);
+        const uint32_t s[2] = {static_cast<uint32_t>(x), static_cast<uint32_t>(x >> 32)};
+        st_bits<1>(c + e, quant_pair<SRC, F8, true>(s, 0, k, m));
+    });
 }
 
 // One kernel per source type; the format (fmt, uniform) picks one of two bodies at the top, so both formats share
@@ -178,14 +129,9 @@ template <int SRC>
 __global__ void fp8_quant_vec(const void* A, void* C, size_t n, size_t head, size_t ngroups, int unroll,
                               int prefetch_first, int fmt, int k, double* amax)
 {
-    constexpr int ES = dt_traits<SRC>::size;
     const unsigned char* a = static_cast<const unsigned char*>(A);
     unsigned char* c = static_cast<unsigned char*>(C);
-    if (prefetch_first && threadIdx.x == 0) {
-        const size_t tile = static_cast<size_t>(blockDim.x) * unroll, g0 = blockIdx.x * tile;
-        if (g0 < ngroups)
-            bulk_prefetch_l2(a + (head + g0 * 16) * ES, static_cast<uint32_t>((ngroups - g0 < tile ? ngroups - g0 : tile) * 16 * ES));
-    }
+    prefetch_first_tile<16, dt_traits<SRC>::size>(prefetch_first, a, head, ngroups, unroll);
     pdl_wait();
 
     amax_bits_t<SRC> m = 0;
@@ -235,60 +181,22 @@ __device__ __forceinline__ u32x4 dequant_slice(unsigned long long v, int k)
     return u32x4{d[0], d[1], d[2], d[3]};
 }
 
-// W FP8 bytes at a (W-byte aligned), as the low bytes of one word.
-template <int W>
-__device__ __forceinline__ unsigned long long ld_fp8(const unsigned char* a)
-{
-    if constexpr (W == 8) return *reinterpret_cast<const unsigned long long*>(a);
-    else if constexpr (W == 4) return *reinterpret_cast<const uint32_t*>(a);
-    else return *reinterpret_cast<const unsigned short*>(a);
-}
-
-// Tiles of blockDim.x * U slices, grid-strided; thread t takes slices t + j blockDim.x of a tile, so lane-
-// consecutive 16-byte stores.  A full tile issues its U loads before its first store.
-template <int F8, int DST, int U>
-__device__ __forceinline__ void dequant_tiles(const unsigned char* a, unsigned char* c, size_t nslices, int k)
-{
-    constexpr int W = 16 / dt_traits<DST>::size;
-    const size_t tile = static_cast<size_t>(blockDim.x) * U;
-    for (size_t t = blockIdx.x; t * tile < nslices; t += gridDim.x) {
-        const size_t s0 = t * tile + threadIdx.x;
-        if ((t + 1) * tile <= nslices) {
-            unsigned long long in[U];
-#pragma unroll
-            for (int j = 0; j < U; ++j) in[j] = ld_fp8<W>(a + (s0 + static_cast<size_t>(j) * blockDim.x) * W);
-#pragma unroll
-            for (int j = 0; j < U; ++j)
-                stg128_bits<ST_NA>(c + (s0 + static_cast<size_t>(j) * blockDim.x) * 16, dequant_slice<F8, DST>(in[j], k));
-        } else {
-#pragma unroll
-            for (int j = 0; j < U; ++j) {
-                const size_t s = s0 + static_cast<size_t>(j) * blockDim.x;
-                if (s < nslices) stg128_bits<ST_NA>(c + s * 16, dequant_slice<F8, DST>(ld_fp8<W>(a + s * W), k));
-            }
-        }
-    }
-}
-
-// Dequantize's body after the dependency wait: elements [head, head + 16 ngroups) are the vector body (sizeof DST
-// slices per group of 16), the others go through the grid-stride scalar loop, as in quant_body.
+// Dequantize's body after the dependency wait: elements [head, head + 16 ngroups) are the vector body, whose units are
+// slices of W = 16 / sizeof DST elements (sizeof DST per group of 16), so lane-consecutive 16-byte stores; the others
+// go through cast_edges.
 template <int F8, int DST>
 __device__ __forceinline__ void dequant_body(const unsigned char* a, unsigned char* c, size_t n, size_t head,
                                              size_t ngroups, int unroll, int k)
 {
-    constexpr int ES = dt_traits<DST>::size;
-    if (unroll == 2) dequant_tiles<F8, DST, 2>(a + head, c + head * ES, ngroups * ES, k);
-    else dequant_tiles<F8, DST, 1>(a + head, c + head * ES, ngroups * ES, k);
-
-    const size_t body_end = head + ngroups * 16, edges = head + (n - body_end);
-    const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
-    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < edges; i += stride) {
-        const size_t e = i < head ? i : body_end + (i - head);
-        const u32x4 r = dequant_slice<F8, DST>(a[e], k);
-        if constexpr (ES == 8) *reinterpret_cast<unsigned long long*>(c + e * 8) = r.x | (static_cast<unsigned long long>(r.y) << 32);
-        else if constexpr (ES == 4) *reinterpret_cast<uint32_t*>(c + e * 4) = r.x;
-        else *reinterpret_cast<unsigned short*>(c + e * 2) = static_cast<unsigned short>(r.x);
-    }
+    constexpr int ES = dt_traits<DST>::size, W = 16 / ES;
+    const unsigned char* ab = a + head;
+    unsigned char* cb = c + head * ES;
+    cast_tiles(unroll, ngroups * ES, [=](size_t u) { return ld_bits<W>(ab + u * W); },
+               [=](size_t u, unsigned long long v) { stg128_bits<ST_NA>(cb + u * 16, dequant_slice<F8, DST>(v, k)); });
+    cast_edges(n, head, head + ngroups * 16, [=](size_t e) {
+        const u32x4 r = dequant_slice<F8, DST>(ld_bits<1>(a + e), k);
+        st_bits<ES>(c + e * ES, r.x | static_cast<unsigned long long>(r.y) << 32);
+    });
 }
 
 // One kernel per destination type, the format picked at the top as in fp8_quant_vec.
@@ -299,12 +207,7 @@ __global__ void fp8_dequant_vec(const void* A, void* C, size_t n, size_t head, s
     constexpr int ES = dt_traits<DST>::size;
     const unsigned char* a = static_cast<const unsigned char*>(A);
     unsigned char* c = static_cast<unsigned char*>(C);
-    const size_t nslices = ngroups * ES;
-    if (prefetch_first && threadIdx.x == 0) {
-        const size_t tile = static_cast<size_t>(blockDim.x) * unroll, s0 = blockIdx.x * tile;
-        if (s0 < nslices)
-            bulk_prefetch_l2(a + head + s0 * (16 / ES), static_cast<uint32_t>((nslices - s0 < tile ? nslices - s0 : tile) * (16 / ES)));
-    }
+    prefetch_first_tile<16 / ES, 1>(prefetch_first, a, head, ngroups * ES, unroll);
     pdl_wait();
 
     if (fmt == F8_E4M3) dequant_body<F8_E4M3, DST>(a, c, n, head, ngroups, unroll, k);

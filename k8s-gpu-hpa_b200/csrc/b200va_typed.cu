@@ -106,62 +106,63 @@ int launch_dot_typed(const void* dA, const void* dB, size_t n, double* ws, cudaS
                          ws, prefetch_first);
 }
 
-// b200va_convert between two distinct types: one convert_vec launch.  The head is the smallest h < G at
-// which A and C both sit on a 16-byte boundary; with none (mixed phase) head = n, and the kernel's scalar
-// loop takes every element.  The geometry is one form for the HBM class (the wider operand >= 128 MiB) and
-// one below it, neither measured yet.
+// The launch of a cast kernel (convert_vec, fp8_quant_vec, fp8_dequant_vec) over n elements of esa bytes at a to
+// esc bytes at c.  A group is G = 16 / min(esa, esc) elements, one 16-byte vector on the narrow side, and a thread's
+// unit of work is 1 / units_per_group of a group.  The head is the smallest h < G at which A and C both sit on a
+// 16-byte boundary; with none (mixed phase) head = n, and the kernel's edge loop takes every element.  The geometry
+// follows the HBM class of the wider operand: 512 x 2 with the L2 prefetch there, 256 x 1 below it (neither
+// measured yet).
+struct cast_plan {
+    size_t head, ngroups;
+    unsigned grid, threads;
+    int unroll, prefetch_first;
+};
+
+cast_plan plan_cast(uintptr_t a, size_t esa, uintptr_t c, size_t esc, size_t n, size_t units_per_group)
+{
+    const size_t G = 16 / std::min(esa, esc);
+    cast_plan p;
+    p.head = n;
+    for (size_t h = head_peel(a, esa); h < G; h += 16 / esa)
+        if (((c + h * esc) & 15u) == 0) { p.head = h; break; }
+    if (p.head > n) p.head = n;
+    p.ngroups = (n - p.head) / G;
+    const size_t units = p.ngroups * units_per_group, edges = n - p.ngroups * G;
+    const bool hbm = hbm_class(n, std::max(esa, esc));
+    p.threads = hbm ? 512 : 256;
+    p.unroll = hbm ? 2 : 1;
+    p.prefetch_first = hbm ? 1 : 0;
+    const size_t tile = static_cast<size_t>(p.threads) * p.unroll;
+    const size_t blocks = std::max((units + tile - 1) / tile, (edges + p.threads - 1) / p.threads);
+    p.grid = static_cast<unsigned>(std::max<size_t>(std::min<size_t>(blocks, 0x7fffffff), 1));
+    return p;
+}
+
+// b200va_convert between two distinct types: one convert_vec launch, a group per unit.
 template <int SRC, int DST>
 int launch_convert_typed(const void* dA, void* dC, size_t n, cudaStream_t st)
 {
-    using S = convert_shape<SRC, DST>;
-    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC);
-    size_t head = n;
-    for (size_t h = head_peel(a, S::ESS); h < static_cast<size_t>(S::G); h += 16 / S::ESS)
-        if (((c + h * S::ESD) & 15u) == 0) { head = h; break; }
-    if (head > n) head = n;
-    const size_t ngroups = (n - head) / S::G;
-    const size_t edges = n - ngroups * S::G;
-    const bool hbm = hbm_class(n, std::max(S::ESS, S::ESD));
-    const unsigned threads = hbm ? 512 : 256;
-    const int unroll = hbm ? 2 : 1;
-    const int prefetch_first = hbm ? 1 : 0;
-    const size_t tile = static_cast<size_t>(threads) * unroll;
-    const size_t blocks = std::max((ngroups + tile - 1) / tile, (edges + threads - 1) / threads);
-    const unsigned grid = static_cast<unsigned>(std::max<size_t>(std::min<size_t>(blocks, 0x7fffffff), 1));
-    return launch_kernel(convert_vec<SRC, DST>, grid, threads, 0, st, pdl_enabled(), dA, dC, n, head, ngroups, unroll,
-                         prefetch_first);
+    const cast_plan p = plan_cast(reinterpret_cast<uintptr_t>(dA), dt_traits<SRC>::size, reinterpret_cast<uintptr_t>(dC),
+                                  dt_traits<DST>::size, n, 1);
+    return launch_kernel(convert_vec<SRC, DST>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
+                         p.unroll, p.prefetch_first);
 }
 
 // b200va_quantize_fp8 (QUANT: T -> fmt) and b200va_dequantize_fp8 (fmt -> T): one fp8_quant_vec<T> or
-// fp8_dequant_vec<T> launch, the format passed to the kernel; planned as convert_vec's with G = 16.  The head is
-// the smallest h < 16 at which A and C both sit on a 16-byte boundary (head = n in mixed phase).  A thread's unit of work is a group of 16 when quantizing and a
-// 16-byte output slice (sizeof T per group) when dequantizing.  The geometry follows the HBM class of the wider
-// operand (T), as convert's does: 512 x 2 with the L2 prefetch there, 256 x 1 below it.
+// fp8_dequant_vec<T> launch, the format passed to the kernel.  A unit is a group of 16 when quantizing and a 16-byte
+// output slice (sizeof T per group) when dequantizing.
 template <bool QUANT, int T>
 int launch_fp8_typed(const void* dA, void* dC, size_t n, int fmt, int k, double* amax, cudaStream_t st)
 {
-    constexpr size_t ES = dt_traits<T>::size, ESA = QUANT ? ES : 1, ESC = QUANT ? 1 : ES;
-    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC);
-    size_t head = n;
-    for (size_t h = head_peel(a, ESA); h < 16; h += 16 / ESA)
-        if (((c + h * ESC) & 15u) == 0) { head = h; break; }
-    if (head > n) head = n;
-    const size_t ngroups = (n - head) / 16;
-    const size_t units = QUANT ? ngroups : ngroups * ES;
-    const size_t edges = n - ngroups * 16;
-    const bool hbm = hbm_class(n, ES);
-    const unsigned threads = hbm ? 512 : 256;
-    const int unroll = hbm ? 2 : 1;
-    const int prefetch_first = hbm ? 1 : 0;
-    const size_t tile = static_cast<size_t>(threads) * unroll;
-    const size_t blocks = std::max((units + tile - 1) / tile, (edges + threads - 1) / threads);
-    const unsigned grid = static_cast<unsigned>(std::max<size_t>(std::min<size_t>(blocks, 0x7fffffff), 1));
+    constexpr size_t ES = dt_traits<T>::size;
+    const cast_plan p = plan_cast(reinterpret_cast<uintptr_t>(dA), QUANT ? ES : 1, reinterpret_cast<uintptr_t>(dC),
+                                  QUANT ? 1 : ES, n, QUANT ? 1 : ES);
     if constexpr (QUANT)
-        return launch_kernel(fp8_quant_vec<T>, grid, threads, 0, st, pdl_enabled(), dA, dC, n, head, ngroups, unroll,
-                             prefetch_first, fmt, k, amax);
+        return launch_kernel(fp8_quant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
+                             p.unroll, p.prefetch_first, fmt, k, amax);
     else
-        return launch_kernel(fp8_dequant_vec<T>, grid, threads, 0, st, pdl_enabled(), dA, dC, n, head, ngroups, unroll,
-                             prefetch_first, fmt, k);
+        return launch_kernel(fp8_dequant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
+                             p.unroll, p.prefetch_first, fmt, k);
 }
 
 // The argument rules the two FP8 entry points share, after the dtype and format codes: scale_exp in [-126, 126],

@@ -114,23 +114,64 @@ class Loop:
         self.close()
 
 
-_TORCH_DT = {"f32": "float32", "f64": "float64", "f16": "float16", "bf16": "bfloat16"}
+_FLOAT = {"f32": "float32", "f64": "float64", "f16": "float16", "bf16": "bfloat16"}
+_FP8 = {"e4m3": "float8_e4m3fn", "e5m2": "float8_e5m2"}
+
+
+def _resolve(dtype, names: dict, codes: dict, what: str):
+    """(torch dtype, ABI code) of a dtype given as a torch dtype or by its short name in ``names``."""
+    torch = _torch()
+    dtypes = {getattr(torch, v): k for k, v in names.items()}
+    if isinstance(dtype, str):
+        if dtype not in names:
+            raise TypeError(f"{what} must be one of {sorted(names)}, got {dtype!r}")
+        dtype = getattr(torch, names[dtype])
+    if dtype not in dtypes:
+        raise TypeError(f"{what} must be one of {'/'.join(names.values())}, got {dtype}")
+    return dtype, codes[dtypes[dtype]]
+
+
+def _float_dtype(dtype):
+    """(torch dtype, B200VA_DT_* code) of f32/f64/f16/bf16 given as a torch dtype or "f32"/"f64"/"f16"/"bf16"."""
+    return _resolve(dtype, _FLOAT, capi.DTYPES, "dtype")
+
+
+def _fp8_format(fmt):
+    """(torch dtype, B200VA_F8_* code) of an FP8 format given as a torch dtype or "e4m3" / "e5m2"."""
+    return _resolve(fmt, _FP8, capi.F8, "fmt")
+
+
+def _operand(t, name: str, resolve=_float_dtype) -> int:
+    """The ABI code of a contiguous CUDA tensor whose dtype ``resolve`` accepts (default f32/f64/f16/bf16)."""
+    torch = _torch()
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or not t.is_contiguous():
+        raise TypeError(f"{name} must be a contiguous CUDA tensor")
+    return resolve(t.dtype)[1]
+
+
+def _like(t, dtype, a, name: str):
+    """``t``, checked to be a contiguous tensor of ``dtype`` with a's length on a's device."""
+    torch = _torch()
+    if (not isinstance(t, torch.Tensor) or t.dtype != dtype or t.numel() != a.numel() or t.device != a.device
+            or not t.is_contiguous()):
+        raise TypeError(f"{name} must be a contiguous tensor of {dtype} with a's length on a's device")
+    return t
+
+
+def _out(out, dtype, a):
+    """``out`` checked by _like, or a new tensor of ``dtype`` shaped like a on a's device."""
+    return _torch().empty(a.shape, dtype=dtype, device=a.device) if out is None else _like(out, dtype, a, "out")
 
 
 def stream(op: str, a, b=None, out=None, *, scalar: float = 0.0, stream=None):
     """STREAM-style op (copy | scale | add | triad) on CUDA tensors of f32/f64/f16/bf16
     through b200va_stream.  Asynchronous on the current stream."""
-    torch = _torch()
-    names = {getattr(torch, v): k for k, v in _TORCH_DT.items()}
-    if not a.is_cuda or a.dtype not in names or not a.is_contiguous():
-        raise TypeError("a must be a contiguous CUDA tensor of float32/float64/float16/bfloat16")
-    if out is None:
-        out = torch.empty_like(a)
-    for t in (b, out):
-        if t is not None and (t.dtype != a.dtype or t.numel() != a.numel() or not t.is_cuda or not t.is_contiguous()):
-            raise TypeError("operands must match a in dtype, length and device")
-    with torch.cuda.device(a.device):
-        check(lib.b200va_stream(capi.OPS[op], capi.DTYPES[names[a.dtype]], a.data_ptr(), b.data_ptr() if b is not None else None,
+    code = _operand(a, "a")
+    if b is not None:
+        _like(b, a.dtype, a, "b")
+    out = _out(out, a.dtype, a)
+    with _torch().cuda.device(a.device):
+        check(lib.b200va_stream(capi.OPS[op], code, a.data_ptr(), b.data_ptr() if b is not None else None,
                                 out.data_ptr(), a.numel(), float(scalar), _stream_ptr(stream)), "b200va_stream")
     return out
 
@@ -140,48 +181,11 @@ def convert(a, dtype, out=None, *, stream=None):
     through b200va_convert: round-to-nearest-even, no FTZ, overflow to inf; the same dtype is a bit copy.
     ``out``: a contiguous CUDA tensor of ``dtype`` with a's length on a's device (it may be ``a`` itself when
     both element sizes are equal), else a new one.  Asynchronous on the current stream."""
-    torch = _torch()
-    names = {getattr(torch, v): k for k, v in _TORCH_DT.items()}
-    if not isinstance(a, torch.Tensor) or not a.is_cuda or a.dtype not in names or not a.is_contiguous():
-        raise TypeError("a must be a contiguous CUDA tensor of float32/float64/float16/bfloat16")
-    if isinstance(dtype, str):
-        if dtype not in _TORCH_DT:
-            raise TypeError(f"dtype must be one of {sorted(_TORCH_DT)}, got {dtype!r}")
-        dtype = getattr(torch, _TORCH_DT[dtype])
-    if dtype not in names:
-        raise TypeError(f"dtype must be float32/float64/float16/bfloat16, got {dtype}")
-    if out is None:
-        out = torch.empty(a.shape, dtype=dtype, device=a.device)
-    elif (not isinstance(out, torch.Tensor) or out.dtype != dtype or out.numel() != a.numel() or out.device != a.device
-          or not out.is_contiguous()):
-        raise TypeError("out must be a contiguous tensor of dtype with a's length on a's device")
-    with torch.cuda.device(a.device):
-        check(lib.b200va_convert(capi.DTYPES[names[a.dtype]], a.data_ptr(), capi.DTYPES[names[dtype]], out.data_ptr(),
-                                 a.numel(), _stream_ptr(stream)), "b200va_convert")
-    return out
-
-
-def _fp8_format(fmt):
-    """(torch dtype, B200VA_F8_* code) of an FP8 format given as a torch dtype or "e4m3" / "e5m2"."""
-    torch = _torch()
-    dtypes = {"e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
-    if isinstance(fmt, str):
-        if fmt not in dtypes:
-            raise TypeError(f"fmt must be one of {sorted(dtypes)}, got {fmt!r}")
-        fmt = dtypes[fmt]
-    codes = {v: capi.F8[k] for k, v in dtypes.items()}
-    if fmt not in codes:
-        raise TypeError(f"fmt must be torch.float8_e4m3fn or torch.float8_e5m2, got {fmt}")
-    return fmt, codes[fmt]
-
-
-def _fp8_out(out, dtype, a):
-    torch = _torch()
-    if out is None:
-        return torch.empty(a.shape, dtype=dtype, device=a.device)
-    if (not isinstance(out, torch.Tensor) or out.dtype != dtype or out.numel() != a.numel() or out.device != a.device
-            or not out.is_contiguous()):
-        raise TypeError("out must be a contiguous tensor of the result dtype with a's length on a's device")
+    src = _operand(a, "a")
+    dtype, dst = _float_dtype(dtype)
+    out = _out(out, dtype, a)
+    with _torch().cuda.device(a.device):
+        check(lib.b200va_convert(src, a.data_ptr(), dst, out.data_ptr(), a.numel(), _stream_ptr(stream)), "b200va_convert")
     return out
 
 
@@ -193,17 +197,15 @@ def quantize_fp8(a, fmt, *, scale_exp: int = 0, amax=None, out=None, stream=None
     contiguous CUDA tensor of the FP8 dtype with a's length on a's device, else a new one.  Asynchronous on the
     current stream."""
     torch = _torch()
-    names = {getattr(torch, v): k for k, v in _TORCH_DT.items()}
-    if not isinstance(a, torch.Tensor) or not a.is_cuda or a.dtype not in names or not a.is_contiguous():
-        raise TypeError("a must be a contiguous CUDA tensor of float32/float64/float16/bfloat16")
+    src = _operand(a, "a")
     dtype, code = _fp8_format(fmt)
-    out = _fp8_out(out, dtype, a)
+    out = _out(out, dtype, a)
     if amax is not None and (not isinstance(amax, torch.Tensor) or amax.dtype != torch.float64 or amax.numel() != 1
                              or amax.device != a.device):
         raise TypeError("amax must be a one-element float64 tensor on a's device")
     with torch.cuda.device(a.device):
-        check(lib.b200va_quantize_fp8(capi.DTYPES[names[a.dtype]], a.data_ptr(), code, out.data_ptr(), a.numel(),
-                                      int(scale_exp), amax.data_ptr() if amax is not None else None, _stream_ptr(stream)),
+        check(lib.b200va_quantize_fp8(src, a.data_ptr(), code, out.data_ptr(), a.numel(), int(scale_exp),
+                                      amax.data_ptr() if amax is not None else None, _stream_ptr(stream)),
               "b200va_quantize_fp8")
     return out
 
@@ -213,21 +215,12 @@ def dequantize_fp8(a, dtype, *, scale_exp: int = 0, out=None, stream=None):
     (torch.float32/float64/float16/bfloat16, or "f32"/"f64"/"f16"/"bf16") by b200va_dequantize_fp8: round-to-nearest-
     even, no FTZ, overflow to inf.  ``out``: a contiguous CUDA tensor of ``dtype`` with a's length on a's device, else
     a new one.  Asynchronous on the current stream."""
-    torch = _torch()
-    names = {getattr(torch, v): k for k, v in _TORCH_DT.items()}
-    if not isinstance(a, torch.Tensor) or not a.is_cuda or not a.is_contiguous():
-        raise TypeError("a must be a contiguous CUDA tensor of float8_e4m3fn/float8_e5m2")
-    _, code = _fp8_format(a.dtype)
-    if isinstance(dtype, str):
-        if dtype not in _TORCH_DT:
-            raise TypeError(f"dtype must be one of {sorted(_TORCH_DT)}, got {dtype!r}")
-        dtype = getattr(torch, _TORCH_DT[dtype])
-    if dtype not in names:
-        raise TypeError(f"dtype must be float32/float64/float16/bfloat16, got {dtype}")
-    out = _fp8_out(out, dtype, a)
-    with torch.cuda.device(a.device):
-        check(lib.b200va_dequantize_fp8(code, a.data_ptr(), capi.DTYPES[names[dtype]], out.data_ptr(), a.numel(),
-                                        int(scale_exp), _stream_ptr(stream)), "b200va_dequantize_fp8")
+    code = _operand(a, "a", _fp8_format)
+    dtype, dst = _float_dtype(dtype)
+    out = _out(out, dtype, a)
+    with _torch().cuda.device(a.device):
+        check(lib.b200va_dequantize_fp8(code, a.data_ptr(), dst, out.data_ptr(), a.numel(), int(scale_exp),
+                                        _stream_ptr(stream)), "b200va_dequantize_fp8")
     return out
 
 
@@ -238,12 +231,8 @@ def dot(a, b, *, out=None, workspace=None, stream=None):
     write the result into (its first element); ``workspace``: a CUDA tensor of at least
     b200va_dot_workspace_bytes(n) bytes, else one is taken from the torch allocator for this call."""
     torch = _torch()
-    names = {getattr(torch, v): k for k, v in _TORCH_DT.items()}
-    for name, t in (("a", a), ("b", b)):
-        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype not in names or not t.is_contiguous():
-            raise TypeError(f"{name} must be a contiguous CUDA tensor of float32/float64/float16/bfloat16")
-    if b.dtype != a.dtype or b.numel() != a.numel() or b.device != a.device:
-        raise TypeError("a and b must match in dtype, length and device")
+    code = _operand(a, "a")
+    _like(b, a.dtype, a, "b")
     n = a.numel()
     need = lib.b200va_dot_workspace_bytes(n)
     if out is None:
@@ -259,7 +248,7 @@ def dot(a, b, *, out=None, workspace=None, stream=None):
             # allocated on the stream the call runs on, so the allocator reuses it only after that stream's work
             with torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream()):
                 workspace = torch.empty(max(need, 8), dtype=torch.uint8, device=a.device)
-        check(lib.b200va_dot(capi.DTYPES[names[a.dtype]], a.data_ptr(), b.data_ptr(), n, out.data_ptr(),
+        check(lib.b200va_dot(code, a.data_ptr(), b.data_ptr(), n, out.data_ptr(),
                              workspace.data_ptr(), workspace.numel() * workspace.element_size(), _stream_ptr(stream)),
               "b200va_dot")
     return out

@@ -266,21 +266,23 @@ def test_f16_to_bf16_beyond_32_bit_offsets():
     assert_matches(c, want, "bf16", "n = 2^32 + 4099")
 
 
-def expected_launch(src, dst, n, a_ptr, c_ptr):
-    """(kernel, grid, block) of launch_convert_typed for these addresses."""
-    ess, esd, G = ES[src], ES[dst], group(src, dst)
-    head, h = n, ((16 - a_ptr % 16) % 16) // ess
+def expected_cast_launch(kernel, esa, esc, n, a_ptr, c_ptr, units_per_group=1):
+    """(kernel, grid, block) of plan_cast (b200va_typed.cu): n elements of esa bytes at a_ptr cast to esc bytes at
+    c_ptr, with units_per_group units of work per group."""
+    G = 16 // min(esa, esc)
+    head, h = n, ((16 - a_ptr % 16) % 16) // esa
     while h < G:
-        if (c_ptr + h * esd) % 16 == 0:
+        if (c_ptr + h * esc) % 16 == 0:
             head = h
             break
-        h += 16 // ess
+        h += 16 // esa
     head = min(head, n)
     ngroups = (n - head) // G
+    units = ngroups * units_per_group
     edges = n - ngroups * G
-    threads, unroll = (512, 2) if n >= hbm_n(src, dst) else (256, 1)
-    blocks = max(-(-ngroups // (threads * unroll)), -(-edges // threads))
-    return f"convert_vec<{DT_CODE[src]},{DT_CODE[dst]}>", max(1, min(blocks, 2 ** 31 - 1)), threads
+    threads, unroll = (512, 2) if n >= (1 << 25) * 4 // max(esa, esc) else (256, 1)
+    blocks = max(-(-units // (threads * unroll)), -(-edges // threads))
+    return kernel, max(1, min(blocks, 2 ** 31 - 1)), threads
 
 
 def test_trace_shows_the_planned_kernels(tmp_path):
@@ -294,7 +296,8 @@ def test_trace_shows_the_planned_kernels(tmp_path):
         for n, oa, oc in ((1000, 0, 0), (hbm_n(src, dst), 0, 0), (1001, 0, 1), (4099, 1, 1)):
             a, c = bufs[src][oa:oa + n], outs[dst][oc:oc + n]
             plan.append((src, dst, a, c))
-            want.append(expected_launch(src, dst, n, a.data_ptr(), c.data_ptr()))
+            want.append(expected_cast_launch(f"convert_vec<{DT_CODE[src]},{DT_CODE[dst]}>", ES[src], ES[dst], n,
+                                             a.data_ptr(), c.data_ptr()))
     for dt in V.DTYPES:
         plan.append((dt, dt, bufs[dt][:1000], outs[dt][:1000]))
         want.append((f"stream_vec<{DT_CODE[dt]},0,1,0,0>", -(-1000 * ES[dt] // 16 // 128), 128))

@@ -37,6 +37,7 @@ if has_gpu():
     from test_gpu_parity import _profiled_kernel_name
     from test_gpu_pdl_chains import LO, M, _chains, _run, env  # noqa: F401  (env: the module-scoped fixture)
     from test_gpu_stream import GUARD, POISON, assert_guards, assert_matches, poisoned, tiled, to_dev
+    from test_gpu_typecast import expected_cast_launch
 
     TORCH = {"f32": torch.float32, "f64": torch.float64, "f16": torch.float16, "bf16": torch.bfloat16}
     TORCH8 = {"e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
@@ -455,26 +456,6 @@ def test_quantize_tail_reads_what_the_writer_wrote(env):
 
 
 # ------------------------------------------------------------------------------------------- trace
-def expected_launch(kind, t, fmt, n, a_ptr, c_ptr):
-    """(kernel, grid, block) of launch_fp8_typed for these addresses."""
-    es = ES[t]
-    esa, esc = (es, 1) if kind == "q" else (1, es)
-    head, h = n, ((16 - a_ptr % 16) % 16) // esa
-    while h < 16:
-        if (c_ptr + h * esc) % 16 == 0:
-            head = h
-            break
-        h += 16 // esa
-    head = min(head, n)
-    ngroups = (n - head) // 16
-    units = ngroups if kind == "q" else ngroups * es
-    edges = n - ngroups * 16
-    threads, unroll = (512, 2) if n >= hbm_n(t) else (256, 1)
-    blocks = max(-(-units // (threads * unroll)), -(-edges // threads))
-    name = f"fp8_quant_vec<{DT_CODE[t]}>" if kind == "q" else f"fp8_dequant_vec<{DT_CODE[t]}>"
-    return name, max(1, min(blocks, 2 ** 31 - 1)), threads
-
-
 def test_trace_shows_the_planned_kernels(tmp_path):
     """Per pair: n = 1000, the HBM class, n = 1001 in mixed phase and an odd n with a head.  Under the profiler the
     kernels after the marker are exactly the planned ones with their grid and block."""
@@ -488,10 +469,12 @@ def test_trace_shows_the_planned_kernels(tmp_path):
         for n, oa, oc in ((1000, 0, 0), (hbm_n(t), 0, 0), (1001, 0, 1), (4099, 1, 1)):
             if kind == "q":
                 a, c = wide[t][oa:oa + n], narrow_out[fmt][oc:oc + n]
+                launch = (f"fp8_quant_vec<{DT_CODE[t]}>", ES[t], 1, n, a.data_ptr(), c.data_ptr())
             else:
                 a, c = narrow[fmt][oa:oa + n], wide_out[t][oc:oc + n]
+                launch = (f"fp8_dequant_vec<{DT_CODE[t]}>", 1, ES[t], n, a.data_ptr(), c.data_ptr(), ES[t])
             plan.append((kind, t, fmt, a, c))
-            want.append(expected_launch(kind, t, fmt, n, a.data_ptr(), c.data_ptr()))
+            want.append(expected_cast_launch(*launch))
     marker = torch.zeros(1, device="cuda")
     amax = _amax_tensor()
     torch.cuda.synchronize()
