@@ -100,6 +100,22 @@ __device__ __forceinline__ void st_bits(unsigned char* p, unsigned long long v)
     else *p = static_cast<unsigned char>(v);
 }
 
+// One element as the words a group holds it in: the ES (2, 4 or 8) bytes at p, ES-aligned, to s[0] and s[1] (the
+// bytes it does not have are 0); and the low ES bytes of lo, hi stored to p.
+template <int ES>
+__device__ __forceinline__ void ld_elem(const unsigned char* p, uint32_t* s)
+{
+    const unsigned long long x = ld_bits<ES>(p);
+    s[0] = static_cast<uint32_t>(x);
+    s[1] = static_cast<uint32_t>(x >> 32);
+}
+
+template <int ES>
+__device__ __forceinline__ void st_elem(unsigned char* p, uint32_t lo, uint32_t hi)
+{
+    st_bits<ES>(p, lo | static_cast<unsigned long long>(hi) << 32);
+}
+
 // V consecutive 16-byte vectors, as a value a tile can hold per unit.
 template <int V>
 struct vecs { u32x4 v[V]; };
@@ -199,11 +215,10 @@ template <int SRC, int DST>
 __device__ __forceinline__ void convert_elem(const unsigned char* a, unsigned char* c)
 {
     using S = convert_shape<SRC, DST>;
-    const unsigned long long x = ld_bits<S::ESS>(a);
-    const uint32_t s[2] = {static_cast<uint32_t>(x), static_cast<uint32_t>(x >> 32)};
-    uint32_t d[2] = {0, 0};
+    uint32_t s[2], d[2] = {0, 0};
+    ld_elem<S::ESS>(a, s);
     convert_words<SRC, DST, 1>(s, d);
-    st_bits<S::ESD>(c, d[0] | static_cast<unsigned long long>(d[1]) << 32);
+    st_elem<S::ESD>(c, d[0], d[1]);
 }
 
 // ---- the kernel -------------------------------------------------------------------------------------

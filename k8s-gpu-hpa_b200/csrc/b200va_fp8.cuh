@@ -28,9 +28,22 @@ namespace b200va {
 
 enum : int { F8_E4M3 = 0, F8_E5M2 = 1, F8_COUNT = 2 };
 
-// 2^k as an f32 / f64, for k in [-126, 126] (a normal number either way).
-__device__ __forceinline__ float pow2_f32(int k) { return __int_as_float((127 + k) << 23); }
-__device__ __forceinline__ double pow2_f64(int k) { return __longlong_as_double(static_cast<long long>(1023 + k) << 52); }
+// The format (fmt, uniform across the launch) to a template argument: f(F8) for the one that matches, so a kernel
+// takes one branch at the top and both formats share it.
+template <class F>
+__device__ __forceinline__ void with_f8(int fmt, F f)
+{
+    if (fmt == F8_E4M3) f(std::integral_constant<int, F8_E4M3>{});
+    else f(std::integral_constant<int, F8_E5M2>{});
+}
+
+// 2^k in DT's arithmetic type (f64 for f64, f32 otherwise), for k in [-126, 126] (a normal number either way).
+template <int DT>
+__device__ __forceinline__ typename dt_traits<DT>::scalar pow2(int k)
+{
+    if constexpr (DT == DT_F64) return __longlong_as_double(static_cast<long long>(1023 + k) << 52);
+    else return __int_as_float((127 + k) << 23);
+}
 
 // Two f32 rounded (RN, saturating at +-max finite) to FP8: lo in bits 0..7, hi in bits 8..15.
 template <int F8>
@@ -79,14 +92,33 @@ __device__ __forceinline__ uint32_t quant_pair(const uint32_t* s, int e0, int k,
         if constexpr (SRC == DT_F64) {
             const double x = elem_f64(s, e0 + j);
             m = max(m, static_cast<unsigned long long>(__double_as_longlong(x)) & 0x7fffffffffffffffull);
-            q[j] = f32_round_odd(__dmul_rn(x, pow2_f64(k)));
+            q[j] = f32_round_odd(__dmul_rn(x, pow2<SRC>(k)));
         } else {
             const float x = elem_f32<SRC>(s, e0 + j);
             m = max(m, __float_as_uint(x) & 0x7fffffffu);
-            q[j] = __fmul_rn(x, pow2_f32(k));
+            q[j] = __fmul_rn(x, pow2<SRC>(k));
         }
     }
     return f8x2_from_f32<F8>(q[0], q[1]);
+}
+
+// One group: the 16 elements in the source words s, scaled by 2^k and rounded to the 16 FP8 bytes of the words d; m
+// takes their magnitudes.
+template <int SRC, int F8>
+__device__ __forceinline__ void quant_group(const uint32_t* s, int k, amax_bits_t<SRC>& m, uint32_t* d)
+{
+#pragma unroll
+    for (int w = 0; w < 4; ++w)
+        d[w] = quant_pair<SRC, F8>(s, 4 * w, k, m) | (quant_pair<SRC, F8>(s, 4 * w + 2, k, m) << 16);
+}
+
+// One element at p (element-size aligned), the same way: its FP8 byte.
+template <int SRC, int F8>
+__device__ __forceinline__ unsigned char quant_elem(const unsigned char* p, int k, amax_bits_t<SRC>& m)
+{
+    uint32_t s[2];
+    ld_elem<dt_traits<SRC>::size>(p, s);
+    return static_cast<unsigned char>(quant_pair<SRC, F8, true>(s, 0, k, m));
 }
 
 template <class T>
@@ -109,22 +141,15 @@ __device__ __forceinline__ void quant_body(const unsigned char* a, unsigned char
     cast_tiles(unroll, ngroups, [=](size_t g) { return ld_vecs<ES>(ab, g); }, [&](size_t g, const vecs<ES>& in) {
         uint32_t s[4 * ES], d[4];
         unpack<ES>(in.v, s);
-#pragma unroll
-        for (int w = 0; w < 4; ++w)
-            d[w] = quant_pair<SRC, F8>(s, 4 * w, k, m) | (quant_pair<SRC, F8>(s, 4 * w + 2, k, m) << 16);
+        quant_group<SRC, F8>(s, k, m, d);
         stg128_bits<ST_NA>(cb + g * 16, u32x4{d[0], d[1], d[2], d[3]});
     });
-    cast_edges(n, head, head + ngroups * 16, [&](size_t e) {
-        const unsigned long long x = ld_bits<ES>(a + e * ES);
-        const uint32_t s[2] = {static_cast<uint32_t>(x), static_cast<uint32_t>(x >> 32)};
-        st_bits<1>(c + e, quant_pair<SRC, F8, true>(s, 0, k, m));
-    });
+    cast_edges(n, head, head + ngroups * 16, [&](size_t e) { c[e] = quant_elem<SRC, F8>(a + e * ES, k, m); });
 }
 
-// One kernel per source type; the format (fmt, uniform) picks one of two bodies at the top, so both formats share
-// a kernel.  unroll (1 or 2) and prefetch_first are the launch's geometry, as in convert_vec.  With amax, each CTA
-// max-accumulates its largest |a_i| (as f64 bits) into *amax with one atomic, after the dependency wait like every
-// other access.
+// One kernel per source type, the format picking one of its two bodies (with_f8).  unroll (1 or 2) and prefetch_first
+// are the launch's geometry, as in convert_vec.  With amax, each CTA max-accumulates its largest |a_i| (as f64 bits)
+// into *amax with one atomic, after the dependency wait like every other access.
 template <int SRC>
 __global__ void fp8_quant_vec(const void* A, void* C, size_t n, size_t head, size_t ngroups, int unroll,
                               int prefetch_first, int fmt, int k, double* amax)
@@ -135,8 +160,7 @@ __global__ void fp8_quant_vec(const void* A, void* C, size_t n, size_t head, siz
     pdl_wait();
 
     amax_bits_t<SRC> m = 0;
-    if (fmt == F8_E4M3) quant_body<SRC, F8_E4M3>(a, c, n, head, ngroups, unroll, k, m);
-    else quant_body<SRC, F8_E5M2>(a, c, n, head, ngroups, unroll, k, m);
+    with_f8(fmt, [&](auto F8) { quant_body<SRC, F8>(a, c, n, head, ngroups, unroll, k, m); });
 
     if (amax) {
         __shared__ unsigned long long part[32];
@@ -157,7 +181,7 @@ __global__ void fp8_quant_vec(const void* A, void* C, size_t n, size_t head, siz
 // W = 16 / sizeof DST FP8 values, in the low bytes of v, to one 16-byte vector of DST scaled by s (a power of two,
 // or a NaN), in f64 for an f64 destination and in f32 otherwise.
 template <int F8, int DST>
-__device__ __forceinline__ u32x4 dequant_slice_scaled(unsigned long long v, typename dt_traits<DST>::scalar s)
+__device__ __forceinline__ u32x4 dequant_slice(unsigned long long v, typename dt_traits<DST>::scalar s)
 {
     uint32_t d[4];
     if constexpr (DST == DT_F64) {
@@ -180,33 +204,34 @@ __device__ __forceinline__ u32x4 dequant_slice_scaled(unsigned long long v, type
     return u32x4{d[0], d[1], d[2], d[3]};
 }
 
-// The same with the per-tensor scale 2^-k.
-template <int F8, int DST>
-__device__ __forceinline__ u32x4 dequant_slice(unsigned long long v, int k)
-{
-    if constexpr (DST == DT_F64) return dequant_slice_scaled<F8, DST>(v, pow2_f64(-k));
-    else return dequant_slice_scaled<F8, DST>(v, pow2_f32(-k));
-}
+// A dequantize unit as a tile holds it: the slice's FP8 bytes and its scale.
+template <int DST>
+struct dequant_unit { unsigned long long v; typename dt_traits<DST>::scalar scale; };
 
-// Dequantize's body after the dependency wait: elements [head, head + 16 ngroups) are the vector body, whose units are
-// slices of W = 16 / sizeof DST elements (sizeof DST per group of 16), so lane-consecutive 16-byte stores; the others
-// go through cast_edges.
-template <int F8, int DST>
+// Dequantize's body after the dependency wait, per tensor and block-scaled: elements [head, head + 16 ngroups) are the
+// vector body, whose units are slices of W = 16 / sizeof DST elements (sizeof DST per group of 16), so lane-consecutive
+// 16-byte stores; the others go through cast_edges.  scale_of(e) is the scale of the slice, or the element, that
+// starts at element e; a tile calls it beside the load of the FP8 bytes, so what it reads is in flight before the
+// tile's first store.
+template <int F8, int DST, class ScaleOf>
 __device__ __forceinline__ void dequant_body(const unsigned char* a, unsigned char* c, size_t n, size_t head,
-                                             size_t ngroups, int unroll, int k)
+                                             size_t ngroups, int unroll, ScaleOf scale_of)
 {
     constexpr int ES = dt_traits<DST>::size, W = 16 / ES;
     const unsigned char* ab = a + head;
     unsigned char* cb = c + head * ES;
-    cast_tiles(unroll, ngroups * ES, [=](size_t u) { return ld_bits<W>(ab + u * W); },
-               [=](size_t u, unsigned long long v) { stg128_bits<ST_NA>(cb + u * 16, dequant_slice<F8, DST>(v, k)); });
+    cast_tiles(unroll, ngroups * ES,
+               [=](size_t u) { return dequant_unit<DST>{ld_bits<W>(ab + u * W), scale_of(head + u * W)}; },
+               [=](size_t u, const dequant_unit<DST>& in) {
+        stg128_bits<ST_NA>(cb + u * 16, dequant_slice<F8, DST>(in.v, in.scale));
+    });
     cast_edges(n, head, head + ngroups * 16, [=](size_t e) {
-        const u32x4 r = dequant_slice<F8, DST>(ld_bits<1>(a + e), k);
-        st_bits<ES>(c + e * ES, r.x | static_cast<unsigned long long>(r.y) << 32);
+        const u32x4 r = dequant_slice<F8, DST>(ld_bits<1>(a + e), scale_of(e));
+        st_elem<ES>(c + e * ES, r.x, r.y);
     });
 }
 
-// One kernel per destination type, the format picked at the top as in fp8_quant_vec.
+// One kernel per destination type, the format picked at the top as in fp8_quant_vec; every slice has the scale 2^-k.
 template <int DST>
 __global__ void fp8_dequant_vec(const void* A, void* C, size_t n, size_t head, size_t ngroups, int unroll,
                                 int prefetch_first, int fmt, int k)
@@ -217,8 +242,9 @@ __global__ void fp8_dequant_vec(const void* A, void* C, size_t n, size_t head, s
     prefetch_first_tile<16 / ES, 1>(prefetch_first, a, head, ngroups * ES, unroll);
     pdl_wait();
 
-    if (fmt == F8_E4M3) dequant_body<F8_E4M3, DST>(a, c, n, head, ngroups, unroll, k);
-    else dequant_body<F8_E5M2, DST>(a, c, n, head, ngroups, unroll, k);
+    with_f8(fmt, [=](auto F8) {
+        dequant_body<F8, DST>(a, c, n, head, ngroups, unroll, [=](size_t) { return pow2<DST>(-k); });
+    });
 }
 
 }  // namespace b200va

@@ -106,6 +106,13 @@ void with_value(int v, F&& f)
 // never L2-resident.  Written as a bound on n so that no n overflows.
 constexpr bool hbm_class(size_t n, size_t es) { return n >= (size_t{1} << 25) * 4 / es; }
 
+// Whether the xbytes bytes at x and the ybytes bytes at y share a byte; a range of no bytes meets nothing.
+inline bool ranges_meet(const void* x, size_t xbytes, const void* y, size_t ybytes)
+{
+    const uintptr_t a = reinterpret_cast<uintptr_t>(x), b = reinterpret_cast<uintptr_t>(y);
+    return xbytes && ybytes && a < b + ybytes && b < a + xbytes;
+}
+
 // C = f(A[, B]) over n elements of `es` bytes: the operands are element-aligned, n is at most 2^40
 // and C either is an input or does not meet it.  `has_b`: B is an operand (otherwise it is ignored).
 inline int check_operands(size_t es, const void* pa, const void* pb, const void* pc, size_t n, bool has_b)
@@ -116,9 +123,9 @@ inline int check_operands(size_t es, const void* pa, const void* pb, const void*
                     c = reinterpret_cast<uintptr_t>(pc);
     if ((a | b | c) & (es - 1)) return B200VA_ERR_ALIGN;
     if (n > (size_t{1} << 40)) return B200VA_ERR_INVALID;
-    const uintptr_t bytes = n * es;
-    auto partial = [&](uintptr_t x) { return x != c && x < c + bytes && c < x + bytes; };
-    if (partial(a) || (has_b && partial(b))) return B200VA_ERR_OVERLAP;
+    const size_t bytes = n * es;
+    auto partial = [&](const void* px) { return px != pc && ranges_meet(px, bytes, pc, bytes); };
+    if (partial(pa) || (has_b && partial(pb))) return B200VA_ERR_OVERLAP;
     return B200VA_OK;
 }
 
@@ -133,7 +140,7 @@ inline int check_convert_operands(size_t esa, const void* pa, size_t esc, const 
     const uintptr_t a = reinterpret_cast<uintptr_t>(pa), c = reinterpret_cast<uintptr_t>(pc);
     if ((a & (esa - 1)) || (c & (esc - 1))) return B200VA_ERR_ALIGN;
     if (n > (size_t{1} << 40)) return B200VA_ERR_INVALID;
-    if (a < c + n * esc && c < a + n * esa) return B200VA_ERR_OVERLAP;
+    if (ranges_meet(pa, n * esa, pc, n * esc)) return B200VA_ERR_OVERLAP;
     return B200VA_OK;
 }
 

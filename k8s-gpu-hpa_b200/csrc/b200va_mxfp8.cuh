@@ -102,9 +102,7 @@ __device__ __forceinline__ void mx_quant_body(const unsigned char* a, unsigned c
 #pragma unroll
         for (int e = 0; e < 16; ++e) m = max(m, finite_mag<SRC>(s, e));
         const int ex = mx_exponent<SRC, F8>(block_max(m, lanes), rule);
-#pragma unroll
-        for (int w = 0; w < 4; ++w)
-            d[w] = quant_pair<SRC, F8>(s, 4 * w, -ex, unused) | (quant_pair<SRC, F8>(s, 4 * w + 2, -ex, unused) << 16);
+        quant_group<SRC, F8>(s, -ex, unused, d);
         if (g < ngroups) {
             stg128_bits<ST_NA>(c + g * 16, u32x4{d[0], d[1], d[2], d[3]});
             if (g % lanes == 0) sc[g / lanes] = static_cast<unsigned char>(ex + 127);
@@ -115,17 +113,13 @@ __device__ __forceinline__ void mx_quant_body(const unsigned char* a, unsigned c
         const size_t e0 = b * block, e1 = e0 + block < n ? e0 + block : n;
         amax_bits_t<SRC> m = 0, unused = 0;
         for (size_t e = e0; e < e1; ++e) {
-            const unsigned long long x = ld_bits<ES>(a + e * ES);
-            const uint32_t s[2] = {static_cast<uint32_t>(x), static_cast<uint32_t>(x >> 32)};
+            uint32_t s[2];
+            ld_elem<ES>(a + e * ES, s);
             m = max(m, finite_mag<SRC>(s, 0));
         }
         const int ex = mx_exponent<SRC, F8>(m, rule);
         sc[b] = static_cast<unsigned char>(ex + 127);
-        for (size_t e = e0; e < e1; ++e) {
-            const unsigned long long x = ld_bits<ES>(a + e * ES);
-            const uint32_t s[2] = {static_cast<uint32_t>(x), static_cast<uint32_t>(x >> 32)};
-            st_bits<1>(c + e, quant_pair<SRC, F8, true>(s, 0, -ex, unused));
-        }
+        for (size_t e = e0; e < e1; ++e) c[e] = quant_elem<SRC, F8>(a + e * ES, -ex, unused);
     });
 }
 
@@ -134,10 +128,7 @@ __device__ __forceinline__ void mx_quant_body(const unsigned char* a, unsigned c
 template <int ES, class F>
 __device__ __forceinline__ void mx_with_pair(int dt, int fmt, F f)
 {
-    auto with_fmt = [&](auto T) {
-        if (fmt == F8_E4M3) f(T, std::integral_constant<int, F8_E4M3>{});
-        else f(T, std::integral_constant<int, F8_E5M2>{});
-    };
+    auto with_fmt = [=](auto T) { with_f8(fmt, [=](auto F8) { f(T, F8); }); };
     if constexpr (ES == 4) with_fmt(std::integral_constant<int, DT_F32>{});
     else if constexpr (ES == 8) with_fmt(std::integral_constant<int, DT_F64>{});
     else if (dt == DT_F16) with_fmt(std::integral_constant<int, DT_F16>{});
@@ -165,32 +156,13 @@ __global__ void mx_quant_vec(const void* A, void* C, void* S, size_t n, size_t n
 template <int DST>
 __device__ __forceinline__ typename dt_traits<DST>::scalar mx_scale(uint32_t b)
 {
-    if constexpr (DST == DT_F64) return b == 0xffu ? __longlong_as_double(0x7ff8000000000000ll) : pow2_f64(static_cast<int>(b) - 127);
+    if constexpr (DST == DT_F64) return b == 0xffu ? __longlong_as_double(0x7ff8000000000000ll) : pow2<DST>(static_cast<int>(b) - 127);
     else return __uint_as_float(b == 0xffu ? 0x7fc00000u : b == 0u ? 0x00400000u : b << 23);
 }
 
-// A dequantize unit as a tile holds it: the slice's FP8 bytes and its block's scale byte.
-struct mx_slice { unsigned long long v; uint32_t scale; };
-
-// Dequantize's body after the dependency wait.  Elements [0, 16 ngroups) are the vector body, whose units are slices
-// of W = 16 / sizeof DST elements, each inside one block; the others go through cast_edges, element by element.
-template <int DST, int F8>
-__device__ __forceinline__ void mx_dequant_body(const unsigned char* a, const unsigned char* sc, unsigned char* c, size_t n,
-                                                size_t ngroups, int unroll, int block)
-{
-    constexpr int ES = dt_traits<DST>::size, W = 16 / ES;
-    const int shift = 31 - __clz(block);
-    cast_tiles(unroll, ngroups * ES, [=](size_t u) { return mx_slice{ld_bits<W>(a + u * W), sc[(u * W) >> shift]}; },
-               [=](size_t u, const mx_slice& in) {
-        stg128_bits<ST_NA>(c + u * 16, dequant_slice_scaled<F8, DST>(in.v, mx_scale<DST>(in.scale)));
-    });
-    cast_edges(n, 0, ngroups * 16, [=](size_t e) {
-        const u32x4 r = dequant_slice_scaled<F8, DST>(ld_bits<1>(a + e), mx_scale<DST>(sc[e >> shift]));
-        st_bits<ES>(c + e * ES, r.x | static_cast<unsigned long long>(r.y) << 32);
-    });
-}
-
-// One kernel per destination element size, the type and the format picked at the top as in mx_quant_vec.
+// One kernel per destination element size, the type and the format picked at the top as in mx_quant_vec.  The body is
+// fp8_dequant_vec's from element 0 (elements [0, 16 ngroups), each slice inside one block), with the scale of the
+// block an element lies in.
 template <int ES>
 __global__ void mx_dequant_vec(const void* A, const void* S, void* C, size_t n, size_t ngroups, int unroll,
                                int prefetch_first, int dst, int fmt, int block)
@@ -201,7 +173,10 @@ __global__ void mx_dequant_vec(const void* A, const void* S, void* C, size_t n, 
     prefetch_first_tile<16 / ES, 1>(prefetch_first, a, 0, ngroups * ES, unroll);
     pdl_wait();
 
-    mx_with_pair<ES>(dst, fmt, [=](auto DST, auto F8) { mx_dequant_body<DST, F8>(a, sc, c, n, ngroups, unroll, block); });
+    const int shift = 31 - __clz(block);
+    mx_with_pair<ES>(dst, fmt, [=](auto DST, auto F8) {
+        dequant_body<F8, DST>(a, c, n, 0, ngroups, unroll, [=](size_t e) { return mx_scale<DST>(sc[e >> shift]); });
+    });
 }
 
 }  // namespace b200va

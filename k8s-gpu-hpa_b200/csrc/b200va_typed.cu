@@ -126,20 +126,29 @@ void plan_geometry(cast_plan& p, bool hbm, size_t units, size_t edges)
     p.grid = static_cast<unsigned>(std::max<size_t>(std::min<size_t>(blocks, 0x7fffffff), 1));
 }
 
-// The launch of a cast kernel (convert_vec, fp8_quant_vec, fp8_dequant_vec) over n elements of esa bytes at a to
-// esc bytes at c.  A group is G = 16 / min(esa, esc) elements, one 16-byte vector on the narrow side, and a thread's
-// unit of work is 1 / units_per_group of a group.  The head is the smallest h < G at which A and C both sit on a
-// 16-byte boundary; with none (mixed phase) head = n, and the kernel's edge loop takes every element.  The geometry
-// follows the HBM class of the wider operand.
-cast_plan plan_cast(uintptr_t a, size_t esa, uintptr_t c, size_t esc, size_t n, size_t units_per_group)
+// Where the vector body of a cast over n elements of esa bytes at a to esc bytes at c lies (the geometry is not set).
+// A group is G = 16 / min(esa, esc) elements, one 16-byte vector on the narrow side.  The head is the smallest h < G at
+// which A and C both sit on a 16-byte boundary; with none (mixed phase) head = n, and the kernel's edge loop takes
+// every element.
+cast_plan cast_body(uintptr_t a, size_t esa, uintptr_t c, size_t esc, size_t n)
 {
     const size_t G = 16 / std::min(esa, esc);
-    cast_plan p;
+    cast_plan p{};
     p.head = n;
     for (size_t h = head_peel(a, esa); h < G; h += 16 / esa)
         if (((c + h * esc) & 15u) == 0) { p.head = h; break; }
     if (p.head > n) p.head = n;
     p.ngroups = (n - p.head) / G;
+    return p;
+}
+
+// The launch of a cast kernel (convert_vec, fp8_quant_vec, fp8_dequant_vec): the body of cast_body, a thread's unit
+// of work being 1 / units_per_group of a group and every element outside the body an edge item.  The geometry follows
+// the HBM class of the wider operand.
+cast_plan plan_cast(uintptr_t a, size_t esa, uintptr_t c, size_t esc, size_t n, size_t units_per_group)
+{
+    const size_t G = 16 / std::min(esa, esc);
+    cast_plan p = cast_body(a, esa, c, esc, n);
     plan_geometry(p, hbm_class(n, std::max(esa, esc)), p.ngroups * units_per_group, n - p.ngroups * G);
     return p;
 }
@@ -178,34 +187,31 @@ int check_fp8_args(size_t es, const void* dA, size_t esc, const void* dC, size_t
 {
     if (k < -126 || k > 126) return B200VA_ERR_INVALID;
     RC_TRY(check_convert_operands(es, dA, esc, dC, n));
-    const uintptr_t m = reinterpret_cast<uintptr_t>(d_amax), a = reinterpret_cast<uintptr_t>(dA),
-                    c = reinterpret_cast<uintptr_t>(dC);
-    if (m & 7u) return B200VA_ERR_ALIGN;
-    auto meet = [&](uintptr_t x, size_t bytes) { return m && n && m < x + bytes && x < m + 8; };
-    if (meet(a, n * es) || meet(c, n * esc)) return B200VA_ERR_OVERLAP;
+    if (reinterpret_cast<uintptr_t>(d_amax) & 7u) return B200VA_ERR_ALIGN;
+    if (d_amax && (ranges_meet(d_amax, 8, dA, n * es) || ranges_meet(d_amax, 8, dC, n * esc)))
+        return B200VA_ERR_OVERLAP;
     return B200VA_OK;
 }
 
 // b200va_quantize_mxfp8 (QUANT: T -> fmt) and b200va_dequantize_mxfp8 (fmt -> T), T of ES bytes: one mx_quant_vec<ES>
 // or mx_dequant_vec<ES> launch, the type, format, block and rule passed to the kernel.  The vector body runs only
-// with A and C both on a 16-byte boundary at element 0, where groups of 16 and blocks coincide: the whole blocks
-// when quantizing (a unit is a group; each further block is one edge item), the whole groups when dequantizing (a
-// unit is a 16-byte output slice; each further element is one edge item).  Otherwise every block, or element, is
-// an edge item.  The geometry is plan_cast's.
+// with A and C both on a 16-byte boundary at element 0 (cast_body finds no head), where groups of 16 and blocks
+// coincide: the whole blocks when quantizing (a unit is a group; each further block is one edge item), the whole
+// groups when dequantizing (a unit is a 16-byte output slice; each further element is one edge item).  Otherwise
+// every block, or element, is an edge item.  The geometry is plan_cast's.
 template <bool QUANT, int ES>
 int launch_mx_typed(const void* dA, void* dS, void* dC, size_t n, int dt, int fmt, int block, int rule, cudaStream_t st)
 {
-    const bool body = ((reinterpret_cast<uintptr_t>(dA) | reinterpret_cast<uintptr_t>(dC)) & 15u) == 0;
-    const size_t nblocks = (n + block - 1) / block;
-    cast_plan p;
-    p.head = 0;
+    cast_plan p = cast_body(reinterpret_cast<uintptr_t>(dA), QUANT ? ES : 1, reinterpret_cast<uintptr_t>(dC),
+                            QUANT ? 1 : ES, n);
+    if (p.head != 0) p = {};      // no vector body: every block, or element, is an edge item
     if constexpr (QUANT) {
-        p.ngroups = body ? n / block * (block / 16) : 0;
-        plan_geometry(p, hbm_class(n, ES), p.ngroups, nblocks - p.ngroups * 16 / block);
+        const size_t per_block = block / 16;
+        p.ngroups -= p.ngroups % per_block;
+        plan_geometry(p, hbm_class(n, ES), p.ngroups, (n + block - 1) / block - p.ngroups / per_block);
         return launch_kernel(mx_quant_vec<ES>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, dS, n, p.ngroups, p.unroll,
                              p.prefetch_first, dt, fmt, block, rule);
     } else {
-        p.ngroups = body ? n / 16 : 0;
         plan_geometry(p, hbm_class(n, ES), p.ngroups * ES, n - p.ngroups * 16);
         return launch_kernel(mx_dequant_vec<ES>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dS, dC, n, p.ngroups, p.unroll,
                              p.prefetch_first, dt, fmt, block);
@@ -220,11 +226,8 @@ int check_mx_args(size_t es, const void* dA, size_t esc, const void* dC, const v
     if (block != 32 && block != 64 && block != 128) return B200VA_ERR_INVALID;
     if (n && !dS) return B200VA_ERR_INVALID;
     RC_TRY(check_convert_operands(es, dA, esc, dC, n));
-    const uintptr_t s = reinterpret_cast<uintptr_t>(dS), a = reinterpret_cast<uintptr_t>(dA),
-                    c = reinterpret_cast<uintptr_t>(dC);
     const size_t sbytes = b200va_mxfp8_scale_bytes(n, block);
-    auto meet = [&](uintptr_t x, size_t bytes) { return n && s < x + bytes && x < s + sbytes; };
-    if (meet(a, n * es) || meet(c, n * esc)) return B200VA_ERR_OVERLAP;
+    if (ranges_meet(dS, sbytes, dA, n * es) || ranges_meet(dS, sbytes, dC, n * esc)) return B200VA_ERR_OVERLAP;
     return B200VA_OK;
 }
 
@@ -343,10 +346,9 @@ int b200va_dot(int dtype, const void* dA, const void* dB, size_t n, double* d_ou
     if (n && ((a | b) & (es - 1)) != 0) return B200VA_ERR_ALIGN;
     if ((o & 7u) || (need && (w & 7u))) return B200VA_ERR_ALIGN;
     // what the call writes (d_out, the needed workspace) must not meet what it reads or each other
-    auto meet = [](uintptr_t x, size_t xn, uintptr_t y, size_t yn) { return xn && yn && x < y + yn && y < x + xn; };
     const size_t bytes = n * es;
-    if (meet(o, 8, a, bytes) || meet(o, 8, b, bytes) || meet(o, 8, w, need) || meet(w, need, a, bytes) ||
-        meet(w, need, b, bytes))
+    if (ranges_meet(d_out, 8, dA, bytes) || ranges_meet(d_out, 8, dB, bytes) || ranges_meet(d_out, 8, d_workspace, need) ||
+        ranges_meet(d_workspace, need, dA, bytes) || ranges_meet(d_workspace, need, dB, bytes))
         return B200VA_ERR_OVERLAP;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     double* ws = static_cast<double*>(d_workspace);

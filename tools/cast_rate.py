@@ -1,0 +1,147 @@
+"""Rate of the cast kernels by family, next to the f32 COPY and READ2 ceiling probes, in one process.
+
+    python tools/cast_rate.py [--family convert|fp8|mxfp8|all] [--log2n 28] [--calls 20] [--rounds 3]
+
+Per round, every op of the chosen families is timed at n elements with CUDA events around `calls` back-to-back calls
+(after two warm-up calls), then b200va_probe_f32 COPY (8 n bytes) and READ2 (8 n read) at the same n.  The families
+and the algorithmic bytes of one call:
+  convert  every ordered pair of distinct types of f32, f64, f16, bf16: n * (sizeof SRC + sizeof DST);
+  fp8      per type and format (E4M3, E5M2): quantize without amax, quantize with amax, dequantize back:
+           n * (sizeof T + 1);
+  mxfp8    per type and format, alternated in this order: quantize and dequantize at block 32 and at block 128,
+           n * (sizeof T + 1 + 1 / block); then the two-pass per-tensor recipe they replace, b200va_quantize_fp8 with
+           amax into a scratch output (the pass that finds the scale) followed by the real b200va_quantize_fp8,
+           2 n * (sizeof T + 1) bytes as it runs here ("us" is the time of the pair, "TB/s" counts what the pair moves).
+The card's name, power limit and maximum SM clock are printed first (nvidia-smi), as they are part of every number.
+One JSON line per measurement on stdout.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+SIZE = {"f32": 4, "f64": 8, "f16": 2, "bf16": 2}
+
+
+def card() -> dict:
+    q = "name,power.limit,clocks.max.sm"
+    out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True)
+    name, power, clock = (s.strip() for s in out.stdout.splitlines()[0].split(","))
+    return {"card": name, "power_limit": power, "max_sm_clock": clock}
+
+
+def timed(fn, calls: int) -> float:
+    """Seconds per call: CUDA events around `calls` back-to-back calls after two warm-up calls."""
+    import torch
+
+    fn()
+    fn()
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    start.record()
+    for _ in range(calls):
+        fn()
+    end.record()
+    end.synchronize()
+    return start.elapsed_time(end) / 1e3 / calls
+
+
+# Each family yields (op name, callable, algorithmic bytes per call); its operands live until the next one is asked for.
+def convert_ops(torch, va, n, tdt, f8):
+    for s in tdt:
+        for d in tdt:
+            if s == d:
+                continue
+            a = torch.randn(n, dtype=torch.float32, device="cuda").to(tdt[s])
+            c = torch.empty(n, dtype=tdt[d], device="cuda")
+            yield f"convert {s}->{d}", lambda: va.convert(a, tdt[d], c), n * (SIZE[s] + SIZE[d])
+            del a, c
+
+
+def fp8_ops(torch, va, n, tdt, f8):
+    for s in tdt:
+        a = torch.randn(n, dtype=torch.float32, device="cuda").to(tdt[s])
+        amax = torch.zeros(1, dtype=torch.float64, device="cuda")
+        for f in f8:
+            q = torch.empty(n, dtype=f8[f], device="cuda")
+            c = torch.empty(n, dtype=tdt[s], device="cuda")
+            nbytes = n * (SIZE[s] + 1)
+            yield f"quantize {s}->{f}", lambda: va.quantize_fp8(a, f8[f], out=q), nbytes
+            yield f"quantize {s}->{f} amax", lambda: va.quantize_fp8(a, f8[f], amax=amax, out=q), nbytes
+            yield f"dequantize {f}->{s}", lambda: va.dequantize_fp8(q, tdt[s], out=c), nbytes
+            del q, c
+        del a, amax
+
+
+def mxfp8_ops(torch, va, n, tdt, f8):
+    for s in tdt:
+        a = torch.randn(n, dtype=torch.float32, device="cuda").to(tdt[s])
+        amax = torch.zeros(1, dtype=torch.float64, device="cuda")
+        c = torch.empty(n, dtype=tdt[s], device="cuda")
+        for f in f8:
+            q = torch.empty(n, dtype=f8[f], device="cuda")
+            scratch = torch.empty(n, dtype=f8[f], device="cuda")
+            for block in (32, 128):
+                sc = torch.empty(n // block, dtype=torch.uint8, device="cuda")
+                nbytes = n * (SIZE[s] + 1) + n // block
+                yield (f"mx quantize {s}->{f} block {block}",
+                       lambda: va.quantize_mxfp8(a, f8[f], block=block, out=q, scales=sc), nbytes)
+                yield (f"mx dequantize {f}->{s} block {block}",
+                       lambda: va.dequantize_mxfp8(q, sc, tdt[s], block=block, out=c), nbytes)
+                del sc
+
+            def two_pass():
+                va.quantize_fp8(a, f8[f], amax=amax, out=scratch)
+                va.quantize_fp8(a, f8[f], out=q)
+
+            yield f"two-pass per-tensor quantize {s}->{f}", two_pass, 2 * n * (SIZE[s] + 1)
+            del q, scratch
+        del a, amax, c
+
+
+FAMILIES = {"convert": convert_ops, "fp8": fp8_ops, "mxfp8": mxfp8_ops}
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("--family", choices=[*FAMILIES, "all"], default="all")
+    ap.add_argument("--log2n", type=int, default=28)
+    ap.add_argument("--calls", type=int, default=20)
+    ap.add_argument("--rounds", type=int, default=3)
+    args = ap.parse_args()
+
+    import torch
+
+    from k8s_gpu_hpa_b200 import vector_add as va
+
+    if not torch.cuda.is_available():
+        raise SystemExit("cast_rate.py needs a CUDA device")
+    n = 1 << args.log2n
+    print(json.dumps(card()), flush=True)
+    tdt = {"f32": torch.float32, "f64": torch.float64, "f16": torch.float16, "bf16": torch.bfloat16}
+    f8 = {"e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
+    families = list(FAMILIES) if args.family == "all" else [args.family]
+
+    def report(r, op, t, nbytes):
+        print(json.dumps({"round": r, "op": op, "n": n, "us": round(t * 1e6, 1), "TB/s": round(nbytes / t / 1e12, 3)}),
+              flush=True)
+
+    for r in range(args.rounds):
+        for family in families:
+            for op, fn, nbytes in FAMILIES[family](torch, va, n, tdt, f8):
+                report(r, op, timed(fn, args.calls), nbytes)
+        x, y, z = (torch.ones(n, dtype=torch.float32, device="cuda") for _ in range(3))
+        for kind, nbytes in (("copy", 8 * n), ("read2", 8 * n)):
+            report(r, f"probe {kind}", timed(lambda: va.probe(kind, x, y, z), args.calls), nbytes)
+        del x, y, z
+        torch.cuda.empty_cache()
+
+
+if __name__ == "__main__":
+    main()
