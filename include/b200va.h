@@ -351,6 +351,48 @@ int b200va_dequantize_mxfp8(int fp8, const void *dA, const void *dS, int dst_dty
 /* Scale bytes for n elements: ceil(n / block); 0 for n = 0 or a block that is not 32, 64 or 128. */
 size_t b200va_mxfp8_scale_bytes(size_t n, int block);
 
+/* ---- stochastic rounding from f32 (row f4) ------------------------------------------------------
+ * Narrowing that keeps, in expectation, what round-to-nearest drops: an f32 value rounds to one of its two
+ * neighbours in the destination with probability given by its position between them, so an update smaller than
+ * half an ulp of the narrow value survives on average.  The random bits come from a counter-based generator, so the
+ * bytes depend only on the value, the seed and the element's global index.
+ * Random bits.  Element i has the global index m = first + i, taken mod 2^64.  splitmix64(z) is the mixing step of the
+ * counter generator above: z += 0x9E3779B97F4A7C15, z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9,
+ * z = (z ^ (z >> 27)) * 0x94D049BB133111EB, z ^= z >> 31.  key = splitmix64(seed) and w_j = splitmix64(key + j) (mod
+ * 2^64).  r_m is the low 32 bits of w_(m>>1) when m is even and the high 32 bits when m is odd: one hash serves two
+ * adjacent global indices.  Hashing the seed first keeps these bits unrelated to what b200va_fill_ctr_f32 makes from
+ * the same seed.
+ * Rounding.  y = a_i for bf16/f16 and y = a_i * 2^scale_exp for FP8.  D is the destination's set of values, with its
+ * subnormals and with the exponent range unbounded above.  For finite nonzero y: lo is the element of D nearest y
+ * toward zero and hi the next element of D away from zero; f = (|y| - |lo|) / (|hi| - |lo|), in [0, 1), and
+ * t = floor(f * 2^32).  The result is hi if t + r_m >= 2^32, else lo, with y's sign (a zero result is +-0 with y's
+ * sign).  Then bf16/f16: a magnitude beyond max finite is +-inf, and +-inf stays +-inf (b200va_convert's overflow
+ * rule).  FP8: |y| beyond max finite, +-inf included, gives +-max finite (448 / 57344), as b200va_quantize_fp8 does.
+ * +-0 stays +-0; a NaN gives a NaN.  No FTZ on either side: f32 subnormal sources and the destination's subnormals
+ * take part.
+ * Consequences:
+ *   - A y already in D never moves.
+ *   - Where neither overflow nor saturation applies, the expected result differs from y by less than 2^-32 of the
+ *     gap hi - lo.
+ *   - The result depends only on (a_i, seed, first + i, scale_exp, destination): not on n, on where A or C sit, on how
+ *     the array is split across calls (call k with first + offset_k on its slice gives the matching bytes), or on
+ *     graph replay.
+ *   - For f32 -> bf16 with y normal, t is the low 16 bits of y's pattern shifted left by 16, and the rule is the
+ *     familiar idiom: add the high 16 bits of r_m to the f32 pattern and clear its low 16 bits.
+ * Arguments, in this order with these codes, as in b200va_convert / b200va_quantize_fp8:
+ * B200VA_ERR_VARIANT: dst_dtype not B200VA_DT_F16 / B200VA_DT_BF16, or fp8 not a B200VA_F8_* code.
+ * B200VA_ERR_INVALID: scale_exp outside [-126, 126], NULL dA/dC with n > 0, n > 2^40.  B200VA_ERR_ALIGN: dA not
+ * 4-byte aligned, dC not aligned to its element size, d_amax not 8-byte aligned.  B200VA_ERR_OVERLAP: C meets A,
+ * or d_amax meets A or C.  A rejected call writes nothing; n = 0 writes nothing.  d_amax (may be NULL)
+ * max-accumulates max_i |a_i| exactly as in b200va_quantize_fp8.
+ * Asynchronous on `stream`: one kernel launch, no allocation, synchronisation or memset; capturable in a CUDA graph. */
+/* c[i] = a[i] stochastically rounded to dst_dtype (B200VA_DT_F16 or B200VA_DT_BF16) */
+int b200va_convert_sr_f32(const float *dA, int dst_dtype, void *dC, size_t n,
+                          uint64_t seed, uint64_t first, void *stream);
+/* c[i] = sat(SR(a[i] * 2^scale_exp)) to E4M3 / E5M2, d_amax as in b200va_quantize_fp8 (may be NULL) */
+int b200va_quantize_fp8_sr_f32(const float *dA, int fp8, void *dC, size_t n, int scale_exp,
+                               uint64_t seed, uint64_t first, double *d_amax, void *stream);
+
 /* ---- reproducible dot product (row f4) --------------------------------------------------
  * *d_out = sum_i a_i b_i as a binary64 value in device memory, written asynchronously on `stream`
  * (not rounded to the storage type; dtype is a B200VA_DT_* code).  Every operand is widened

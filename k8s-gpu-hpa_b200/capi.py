@@ -118,6 +118,8 @@ _SIGS = {
     "b200va_quantize_mxfp8": (_I, [_I, _P, _I, _P, _P, _SZ, _I, _I, _P]),
     "b200va_dequantize_mxfp8": (_I, [_I, _P, _P, _I, _P, _SZ, _I, _P]),
     "b200va_mxfp8_scale_bytes": (_SZ, [_SZ, _I]),
+    "b200va_convert_sr_f32": (_I, [_P, _I, _P, _SZ, _U64, _U64, _P]),
+    "b200va_quantize_fp8_sr_f32": (_I, [_P, _I, _P, _SZ, _I, _U64, _U64, _P, _P]),
     "b200va_dot_workspace_bytes": (_SZ, [_SZ]),
     "b200va_dot": (_I, [_I, _P, _P, _SZ, _P, _P, _SZ, _P]),
     "b200va_probe_f32": (_I, [_I, _P, _P, _P, _SZ, _P]),

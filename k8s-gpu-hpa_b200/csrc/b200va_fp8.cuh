@@ -129,6 +129,24 @@ __device__ __forceinline__ T warp_max(T v)
     return v;
 }
 
+// The CTA's magnitudes m (every thread's) max-accumulated into *amax as f64 bits with one atomic; called by every
+// thread of the CTA, after the dependency wait like every other access.
+template <int SRC>
+__device__ __forceinline__ void cta_amax(double* amax, amax_bits_t<SRC> m)
+{
+    __shared__ unsigned long long part[32];
+    unsigned long long v;
+    if constexpr (SRC == DT_F64) v = m;
+    else v = static_cast<unsigned long long>(__double_as_longlong(static_cast<double>(__uint_as_float(m)))) & 0x7fffffffffffffffull;
+    v = warp_max(v);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (unsigned w = 1; w < blockDim.x / 32; ++w) v = max(v, part[w]);
+        atomicMax(reinterpret_cast<unsigned long long*>(amax), v);
+    }
+}
+
 // Quantize's body after the dependency wait: elements [head, head + 16 ngroups) are the vector body, one group of 16
 // per unit, on 16-byte boundaries in A and in C; the others go through cast_edges.
 template <int SRC, int F8>
@@ -161,20 +179,7 @@ __global__ void fp8_quant_vec(const void* A, void* C, size_t n, size_t head, siz
 
     amax_bits_t<SRC> m = 0;
     with_f8(fmt, [&](auto F8) { quant_body<SRC, F8>(a, c, n, head, ngroups, unroll, k, m); });
-
-    if (amax) {
-        __shared__ unsigned long long part[32];
-        unsigned long long v;
-        if constexpr (SRC == DT_F64) v = m;
-        else v = static_cast<unsigned long long>(__double_as_longlong(static_cast<double>(__uint_as_float(m)))) & 0x7fffffffffffffffull;
-        v = warp_max(v);
-        if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            for (unsigned w = 1; w < blockDim.x / 32; ++w) v = max(v, part[w]);
-            atomicMax(reinterpret_cast<unsigned long long*>(amax), v);
-        }
-    }
+    if (amax) cta_amax<SRC>(amax, m);
 }
 
 // ---- dequantize -------------------------------------------------------------------------------------------

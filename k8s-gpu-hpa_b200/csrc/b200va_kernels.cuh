@@ -494,11 +494,7 @@ __global__ void probe_copy(const float* A, float* C, size_t nvec)
 // integer converts to binary32 exactly and the scale is a power of two, so both give the same bits.
 __host__ __device__ __forceinline__ float ctr_value(uint64_t z)
 {
-    z += 0x9E3779B97F4A7C15ull;                       // splitmix64
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    z ^= z >> 31;
-    return static_cast<float>(static_cast<uint32_t>(z >> 40)) * 0x1.0p-24f;
+    return static_cast<float>(static_cast<uint32_t>(splitmix64(z) >> 40)) * 0x1.0p-24f;
 }
 
 __global__ void fill_ctr(float* x, size_t n, uint64_t base)

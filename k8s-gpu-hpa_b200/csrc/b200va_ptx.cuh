@@ -260,4 +260,16 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads)
     asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(nthreads) : "memory");
 }
 
+// ---------------------------------------------------------------- counter-based random bits
+// splitmix64's output function (Steele, Lea, Flood 2014): the state step, two multiply-xorshift rounds and a final
+// xorshift.  The one definition behind the counter generator (ctr_value, host and device) and the random bits of
+// the stochastic-rounding casts (b200va_sr.cuh, and the key the host derives from their seed).
+__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t z)
+{
+    z += 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
 }  // namespace b200va

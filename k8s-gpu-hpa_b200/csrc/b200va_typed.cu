@@ -1,9 +1,11 @@
 // b200va_typed.cu -- the STREAM ops (copy, scale, add, triad), the reproducible dot product, the
-// conversions between f32, f64, f16 and bf16, and the FP8 quantize and dequantize, per tensor and block-scaled.
-// The only unit that includes the STREAM, dot, convert and FP8 kernels (b200va_dot.cuh and b200va_mxfp8.cuh, which
-// include b200va_fp8.cuh, b200va_convert.cuh and b200va_stream.cuh).
+// conversions between f32, f64, f16 and bf16, the FP8 quantize and dequantize, per tensor and block-scaled, and the
+// stochastically rounded casts from f32.
+// The only unit that includes the STREAM, dot, convert, FP8 and SR kernels (b200va_dot.cuh, b200va_mxfp8.cuh and
+// b200va_sr.cuh, which include b200va_fp8.cuh, b200va_convert.cuh and b200va_stream.cuh).
 #include "b200va_internal.h"
 #include "b200va_mxfp8.cuh"
+#include "b200va_sr.cuh"
 #include "b200va_dot.cuh"
 
 using namespace b200va;
@@ -193,6 +195,17 @@ int check_fp8_args(size_t es, const void* dA, size_t esc, const void* dC, size_t
     return B200VA_OK;
 }
 
+// b200va_convert_sr_f32 and b200va_quantize_fp8_sr_f32: one sr_cast_vec launch, a group per unit, dst one of SR_*.
+// The key of the random bits is derived from the seed here, once per call.
+int launch_sr(const void* dA, int dst, void* dC, size_t n, int k, uint64_t seed, uint64_t first, double* amax,
+              cudaStream_t st)
+{
+    const size_t esc = dst == SR_F16 || dst == SR_BF16 ? 2 : 1;
+    const cast_plan p = plan_cast(reinterpret_cast<uintptr_t>(dA), 4, reinterpret_cast<uintptr_t>(dC), esc, n, 1);
+    return launch_kernel(sr_cast_vec, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups, p.unroll,
+                         p.prefetch_first, dst, k, splitmix64(seed), first, amax);
+}
+
 // b200va_quantize_mxfp8 (QUANT: T -> fmt) and b200va_dequantize_mxfp8 (fmt -> T), T of ES bytes: one mx_quant_vec<ES>
 // or mx_dequant_vec<ES> launch, the type, format, block and rule passed to the kernel.  The vector body runs only
 // with A and C both on a 16-byte boundary at element 0 (cast_body finds no head), where groups of 16 and blocks
@@ -291,6 +304,28 @@ int b200va_dequantize_fp8(int fp8, const void* dA, int dst_dtype, void* dC, size
         rc = launch_fp8_typed<false, DST>(dA, dC, n, fp8, scale_exp, nullptr, static_cast<cudaStream_t>(stream));
     });
     return rc;
+}
+
+int b200va_convert_sr_f32(const float* dA, int dst_dtype, void* dC, size_t n, uint64_t seed, uint64_t first,
+                          void* stream)
+{
+    if (dst_dtype != DT_F16 && dst_dtype != DT_BF16) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    RC_TRY(check_convert_operands(4, dA, 2, dC, n));
+    if (n == 0) return B200VA_OK;
+    return launch_sr(dA, dst_dtype == DT_F16 ? SR_F16 : SR_BF16, dC, n, 0, seed, first, nullptr,
+                     static_cast<cudaStream_t>(stream));
+}
+
+int b200va_quantize_fp8_sr_f32(const float* dA, int fp8, void* dC, size_t n, int scale_exp, uint64_t seed, uint64_t first,
+                               double* d_amax, void* stream)
+{
+    if (fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    RC_TRY(check_fp8_args(4, dA, 1, dC, n, scale_exp, d_amax));
+    if (n == 0) return B200VA_OK;
+    return launch_sr(dA, fp8 == F8_E4M3 ? SR_E4M3 : SR_E5M2, dC, n, scale_exp, seed, first, d_amax,
+                     static_cast<cudaStream_t>(stream));
 }
 
 size_t b200va_mxfp8_scale_bytes(size_t n, int block)

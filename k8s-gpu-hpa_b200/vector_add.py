@@ -224,6 +224,56 @@ def dequantize_fp8(a, dtype, *, scale_exp: int = 0, out=None, stream=None):
     return out
 
 
+_U64 = (1 << 64) - 1
+
+
+def _sr_source(a) -> None:
+    """The stochastically rounding casts take float32 sources only."""
+    torch = _torch()
+    if not isinstance(a, torch.Tensor) or a.dtype != torch.float32:
+        raise TypeError(f"a must be a float32 tensor, got {getattr(a, 'dtype', type(a).__name__)}")
+    _operand(a, "a")
+
+
+def convert_sr(a, dtype, *, seed: int, offset: int = 0, out=None, stream=None):
+    """float32 ``a`` rounded stochastically to ``dtype`` (torch.float16 / torch.bfloat16, or "f16" / "bf16") by
+    b200va_convert_sr_f32: each element rounds to one of its two neighbours, up with probability equal to its
+    position between them, past max finite to inf.  The random bits depend only on ``seed`` and the global index
+    ``offset + i`` of element i (both taken mod 2^64), so a slice cast with offset equal to its start gives the same
+    bytes as the matching slice of a whole-array call.  ``out``: a contiguous CUDA tensor of ``dtype`` with a's
+    length on a's device, else a new one.  Asynchronous on the current stream."""
+    _sr_source(a)
+    dtype, dst = _float_dtype(dtype)
+    if dst not in (capi.DTYPES["f16"], capi.DTYPES["bf16"]):
+        raise TypeError(f"dtype must be float16 or bfloat16, got {dtype}")
+    out = _out(out, dtype, a)
+    with _torch().cuda.device(a.device):
+        check(lib.b200va_convert_sr_f32(a.data_ptr(), dst, out.data_ptr(), a.numel(), int(seed) & _U64,
+                                        int(offset) & _U64, _stream_ptr(stream)), "b200va_convert_sr_f32")
+    return out
+
+
+def quantize_fp8_sr(a, fmt, *, seed: int, offset: int = 0, scale_exp: int = 0, amax=None, out=None, stream=None):
+    """float32 ``a`` times 2^scale_exp rounded stochastically to FP8 (b200va_quantize_fp8_sr_f32): the random bits and
+    rounding of convert_sr, then saturation at +-max finite (448 for E4M3, 57344 for E5M2), inf included; NaN stays
+    NaN.  ``fmt``: torch.float8_e4m3fn / torch.float8_e5m2 or "e4m3" / "e5m2".  ``amax``: as in quantize_fp8.
+    ``out``: a contiguous CUDA tensor of the FP8 dtype with a's length on a's device, else a new one.  Asynchronous on
+    the current stream."""
+    torch = _torch()
+    _sr_source(a)
+    dtype, code = _fp8_format(fmt)
+    out = _out(out, dtype, a)
+    if amax is not None and (not isinstance(amax, torch.Tensor) or amax.dtype != torch.float64 or amax.numel() != 1
+                             or amax.device != a.device):
+        raise TypeError("amax must be a one-element float64 tensor on a's device")
+    with torch.cuda.device(a.device):
+        check(lib.b200va_quantize_fp8_sr_f32(a.data_ptr(), code, out.data_ptr(), a.numel(), int(scale_exp),
+                                             int(seed) & _U64, int(offset) & _U64,
+                                             amax.data_ptr() if amax is not None else None, _stream_ptr(stream)),
+              "b200va_quantize_fp8_sr_f32")
+    return out
+
+
 def _mx_scales(scales, a, block: int):
     """``scales`` checked to be a contiguous one-byte tensor (uint8, or float8_e8m0fnu where torch has it) of
     b200va_mxfp8_scale_bytes(n, block) elements on a's device, or a new uint8 one."""

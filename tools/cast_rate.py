@@ -1,6 +1,6 @@
 """Rate of the cast kernels by family, next to the f32 COPY and READ2 ceiling probes, in one process.
 
-    python tools/cast_rate.py [--family convert|fp8|mxfp8|all] [--log2n 28] [--calls 20] [--rounds 3]
+    python tools/cast_rate.py [--family convert|fp8|mxfp8|sr|all] [--log2n 28] [--calls 20] [--rounds 3]
 
 Per round, every op of the chosen families is timed at n elements with CUDA events around `calls` back-to-back calls
 (after two warm-up calls), then b200va_probe_f32 COPY (8 n bytes) and READ2 (8 n read) at the same n.  The families
@@ -12,6 +12,10 @@ and the algorithmic bytes of one call:
            n * (sizeof T + 1 + 1 / block); then the two-pass per-tensor recipe they replace, b200va_quantize_fp8 with
            amax into a scratch output (the pass that finds the scale) followed by the real b200va_quantize_fp8,
            2 n * (sizeof T + 1) bytes as it runs here ("us" is the time of the pair, "TB/s" counts what the pair moves).
+  sr       the stochastically rounding casts from f32, each beside its round-to-nearest counterpart: to f16 and bf16,
+           and to E4M3 and E5M2 without and with amax, n * (4 + sizeof DST); then the torch-eager bf16 recipe (a random
+           int32 tensor as large as the input, added to the f32 patterns, masked and cast in separate kernels), counted
+           at the same n * 6 bytes.
 The card's name, power limit and maximum SM clock are printed first (nvidia-smi), as they are part of every number.
 One JSON line per measurement on stdout.
 """
@@ -105,7 +109,34 @@ def mxfp8_ops(torch, va, n, tdt, f8):
         del a, amax, c
 
 
-FAMILIES = {"convert": convert_ops, "fp8": fp8_ops, "mxfp8": mxfp8_ops}
+def sr_ops(torch, va, n, tdt, f8):
+    a = torch.randn(n, dtype=torch.float32, device="cuda")
+    amax = torch.zeros(1, dtype=torch.float64, device="cuda")
+    for d in ("f16", "bf16"):
+        c = torch.empty(n, dtype=tdt[d], device="cuda")
+        nbytes = n * (4 + SIZE[d])
+        yield f"sr convert f32->{d}", lambda: va.convert_sr(a, tdt[d], seed=1, out=c), nbytes
+        yield f"convert f32->{d}", lambda: va.convert(a, tdt[d], c), nbytes
+        del c
+    for f in f8:
+        q = torch.empty(n, dtype=f8[f], device="cuda")
+        nbytes = n * 5
+        yield f"sr quantize f32->{f}", lambda: va.quantize_fp8_sr(a, f8[f], seed=1, out=q), nbytes
+        yield f"quantize f32->{f}", lambda: va.quantize_fp8(a, f8[f], out=q), nbytes
+        yield f"sr quantize f32->{f} amax", lambda: va.quantize_fp8_sr(a, f8[f], seed=1, amax=amax, out=q), nbytes
+        yield f"quantize f32->{f} amax", lambda: va.quantize_fp8(a, f8[f], amax=amax, out=q), nbytes
+        del q
+    c = torch.empty(n, dtype=torch.bfloat16, device="cuda")
+
+    def eager():
+        r = torch.randint(0, 1 << 16, (n,), dtype=torch.int32, device="cuda")
+        c.copy_(((a.view(torch.int32) + r) & -65536).view(torch.float32))
+
+    yield "torch-eager sr f32->bf16", eager, n * 6
+    del a, amax, c
+
+
+FAMILIES = {"convert": convert_ops, "fp8": fp8_ops, "mxfp8": mxfp8_ops, "sr": sr_ops}
 
 
 def main() -> None:
