@@ -1,0 +1,47 @@
+"""The SASS of the built libraries, for the tests that read it (no GPU needed).
+
+The only place the tests run cuobjdump.  A full listing of a library takes seconds (the tune library's the most),
+and dumping one function with `-fun` still reads the whole fatbinary, so each library is dumped once per session
+and split into its functions here.
+"""
+import functools
+import re
+import subprocess
+
+OPCODE = re.compile(r"/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)")
+
+
+@functools.lru_cache(maxsize=None)
+def dump(path: str) -> str:
+    """The whole `cuobjdump -sass` listing of a library."""
+    return subprocess.run(["cuobjdump", "-sass", path], capture_output=True, text=True, check=True).stdout
+
+
+@functools.lru_cache(maxsize=None)
+def functions(path: str) -> dict[str, str]:
+    """Mangled name -> the function's SASS, split from dump(path).  Each name appears once."""
+    parts = re.split(r"^\s*Function : (\S+)\s*$", dump(path), flags=re.M)
+    out = {}
+    for fn, body in zip(parts[1::2], parts[2::2]):
+        assert fn not in out, fn
+        out[fn] = body
+    return out
+
+
+def opcodes(body: str) -> list[str]:
+    """The opcodes of a function's SASS in text order, predicates stripped."""
+    return OPCODE.findall(body)
+
+
+def parse(mangled: str) -> tuple[str, list[int]]:
+    """_ZN6b200va8vadd_vecILi4ELi1ELi0ELi1ELi1EEEv... -> ("vadd_vec", [4, 1, 0, 1, 1])."""
+    m = re.match(r"_ZN6b200va(\d+)", mangled)
+    assert m, mangled
+    name = mangled[m.end():m.end() + int(m.group(1))]
+    targs = re.match(r"I((?:L[a-z]\d+E)+)E", mangled[m.end() + len(name):])
+    return name, [int(v) for v in re.findall(r"L[a-z](\d+)E", targs.group(1))] if targs else []
+
+
+def ptx(path: str) -> str:
+    """The `cuobjdump -lptx` listing of a library: the PTX files it embeds."""
+    return subprocess.run(["cuobjdump", "-lptx", path], capture_output=True, text=True, check=True).stdout

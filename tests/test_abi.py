@@ -12,6 +12,7 @@ import pytest
 
 import k8s_gpu_hpa_b200 as pkg
 import oracle
+import sass
 from conftest import ROOT, has_gpu
 from k8s_gpu_hpa_b200 import capi, vector_add as va
 
@@ -53,22 +54,21 @@ def test_abi_version_and_strerror():
 
 
 def test_library_is_sm90a_only_and_uses_tma_and_the_ticket_scheduler():
-    sass = subprocess.run(["cuobjdump", "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
-    archs = set(re.findall(r"arch = (sm_\w+)", sass))
+    text = sass.dump(capi.LIB_PATH)
+    archs = set(re.findall(r"arch = (sm_\w+)", text))
     assert archs == {"sm_90a"}, archs
-    assert "UBLKCP" in sass            # cp.async.bulk (TMA)
-    assert "SYNCS" in sass             # mbarrier
-    assert "ATOMG.E.ADD" in sass       # the dynamic tile scheduler's ticket counter (K2d, K1d)
-    assert "ACQBULK" in sass and "PREEXIT" in sass           # griddepcontrol.wait / launch_dependents (PDL)
-    assert not re.search(r"[LS][DT]G\.E\S*\.256", sass)     # sm_90 has no 256-bit global access
-    assert re.search(r"LDG\.E\S*\.128", sass) and re.search(r"STG\.E\S*\.128", sass)
-    assert "HMMA" not in sass and "GMMA" not in sass         # a stream, not a contraction
+    assert "UBLKCP" in text            # cp.async.bulk (TMA)
+    assert "SYNCS" in text             # mbarrier
+    assert "ATOMG.E.ADD" in text       # the dynamic tile scheduler's ticket counter (K2d, K1d)
+    assert "ACQBULK" in text and "PREEXIT" in text           # griddepcontrol.wait / launch_dependents (PDL)
+    assert not re.search(r"[LS][DT]G\.E\S*\.256", text)     # sm_90 has no 256-bit global access
+    assert re.search(r"LDG\.E\S*\.128", text) and re.search(r"STG\.E\S*\.128", text)
+    assert "HMMA" not in text and "GMMA" not in text         # a stream, not a contraction
     # "fat binary + PTX" (SURVEY.md 8(f)2): the production library also embeds its compute_90a PTX
-    ptx = subprocess.run(["cuobjdump", "-lptx", capi.LIB_PATH], capture_output=True, text=True).stdout
+    ptx = sass.ptx(capi.LIB_PATH)
     assert "sm_90a.ptx" in ptx, ptx
     # the production library carries the production set, the tune library the whole matrix
-    n_prod = sass.count("Function :")
-    n_tune = subprocess.run(["cuobjdump", "-sass", capi.TUNE_LIB_PATH], capture_output=True, text=True).stdout.count("Function :")
+    n_prod, n_tune = len(sass.functions(capi.LIB_PATH)), len(sass.functions(capi.TUNE_LIB_PATH))
     assert n_prod < 200 < n_tune, (n_prod, n_tune)
 
 
@@ -77,8 +77,7 @@ def test_early_load_variant_issues_its_loads_before_the_dependency_wait():
     and the store after it; the plain kernel waits first."""
     def body(early: int) -> list[str]:
         fn = f"_ZN6b200va8vadd_vecILi4ELi1ELi0ELi1ELi{early}EEEvPKfS2_Pfmmmm"
-        out = subprocess.run(["cuobjdump", "-sass", "-fun", fn, capi.LIB_PATH], capture_output=True, text=True).stdout
-        return re.findall(r"\b(LDG\.E\.128|STG\.E\S*\.128|ACQBULK|UBLKPF\.L2)\b", out)
+        return re.findall(r"\b(LDG\.E\.128|STG\.E\S*\.128|ACQBULK|UBLKPF\.L2)\b", sass.functions(capi.LIB_PATH)[fn])
     early, plain, prefetch = body(1), body(0), body(2)
     assert early and plain and prefetch
     assert early.index("ACQBULK") > [i for i, m in enumerate(early) if m.startswith("LDG")][1]

@@ -13,7 +13,6 @@
 """
 import math
 import re
-import subprocess
 from fractions import Fraction
 
 import numpy as np
@@ -23,6 +22,7 @@ from oracle import convert_exact as V
 from oracle import stream_exact as X
 
 import k8s_gpu_hpa_b200 as pkg  # noqa: F401  (builds nothing; the session fixture has built the library)
+import sass
 from k8s_gpu_hpa_b200 import capi
 
 PAIRS = V.PAIRS
@@ -179,17 +179,13 @@ def test_rounding_patterns_are_the_decisive_low_parts():
 
 
 # ------------------------------------------------------------------------------------------- SASS
-def _sass(fn: str) -> str:
-    return subprocess.run(["cuobjdump", "-sass", "-fun", fn, capi.LIB_PATH], capture_output=True, text=True).stdout
-
-
 def test_convert_kernels_in_the_sass_wait_before_they_release_the_next_launch():
-    sass = subprocess.run(["cuobjdump", "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
-    names = sorted(set(re.findall(r"Function : (_ZN6b200va\d+convert_\w+)", sass)))
+    fns = sass.functions(capi.LIB_PATH)
+    names = sorted(fn for fn in fns if re.match(r"_ZN6b200va\d+convert_\w+", fn))
     assert len(names) == 12, names
     code = {"f32": 0, "f64": 1, "f16": 2, "bf16": 3}
     for fn in names:
-        body = _sass(fn)
+        body = fns[fn]
         src, dst = (k for c in re.search(r"ILi(\d)ELi(\d)E", fn).groups() for k, v in code.items() if v == int(c))
         ops = re.findall(r"\b(LDG\.E\S*|STG\.E\S*|ACQBULK|UBLKPF\.L2|PREEXIT)\b", body)
         assert ops[:2] == ["UBLKPF.L2", "ACQBULK"] and "PREEXIT" in ops[2:], (fn, ops[:4])   # the trigger after the wait

@@ -12,7 +12,6 @@
 import math
 import os
 import re
-import subprocess
 from fractions import Fraction
 
 import numpy as np
@@ -22,6 +21,7 @@ from oracle import dot_exact as D
 from oracle import stream_exact as X
 
 import k8s_gpu_hpa_b200 as pkg
+import sass
 from k8s_gpu_hpa_b200 import capi
 
 DTS = ["f32", "f64", "f16", "bf16"]
@@ -210,15 +210,13 @@ def test_constants_and_workspace_size_match_the_header():
 
 
 def _sass(fn: str) -> list[str]:
-    out = subprocess.run(["cuobjdump", "-sass", "-fun", fn, capi.LIB_PATH], capture_output=True, text=True).stdout
-    return re.findall(r"\b(LDG\.E\S*|LDS\S*|STG\.E\S*|ACQBULK|UBLKPF\.L2|PREEXIT)\b", out)
+    return re.findall(r"\b(LDG\.E\S*|LDS\S*|STG\.E\S*|ACQBULK|UBLKPF\.L2|PREEXIT)\b", sass.functions(capi.LIB_PATH)[fn])
 
 
 def test_dot_kernels_load_nothing_and_release_nothing_before_the_dependency_wait():
     """Before griddepcontrol.wait (ACQBULK) only the two L2 prefetches of the HBM class; the trigger (PREEXIT) and
     every global load and store after it."""
-    sass = subprocess.run(["cuobjdump", "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
-    names = sorted(set(re.findall(r"Function : (_ZN6b200va\d+dot_\w+)", sass)))
+    names = sorted(fn for fn in sass.functions(capi.LIB_PATH) if re.match(r"_ZN6b200va\d+dot_\w+", fn))
     assert len(names) == 9, names                    # dot_vec and dot_scalar per type, dot_final
     for fn in names:
         ops = _sass(fn)

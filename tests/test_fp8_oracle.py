@@ -17,7 +17,6 @@ kernels' SASS.
 """
 import math
 import re
-import subprocess
 from fractions import Fraction
 
 import numpy as np
@@ -29,6 +28,7 @@ from oracle import fp8_exact as F
 from oracle import stream_exact as X
 
 import k8s_gpu_hpa_b200 as pkg  # noqa: F401  (builds nothing; the session fixture has built the library)
+import sass
 from k8s_gpu_hpa_b200 import capi
 
 DTYPES = V.DTYPES
@@ -209,9 +209,7 @@ def test_quantize_then_dequantize_gives_the_fp8_values_scaled_back():
 
 # ------------------------------------------------------------------------------------------- SASS
 def _functions(path: str) -> dict[str, str]:
-    sass = subprocess.run(["cuobjdump", "-sass", path], capture_output=True, text=True, check=True).stdout
-    parts = re.split(r"^\s*Function : (\S+)\s*$", sass, flags=re.M)
-    return {fn: body for fn, body in zip(parts[1::2], parts[2::2]) if re.match(r"_ZN6b200va\d+fp8_", fn)}
+    return {fn: body for fn, body in sass.functions(path).items() if re.match(r"_ZN6b200va\d+fp8_", fn)}
 
 
 @pytest.mark.parametrize("path", ["production", "tune"])

@@ -7,10 +7,8 @@ shards): through size-independent properties -- the order-independent digest of 
 result equals the oracle's digest of A+B (a checksum of checksums over shards), the
 device-side recompute finds no mismatch, commutativity, idempotence, in-place == out-of-place.
 """
-import ctypes as C
 import json
 import os
-import re
 
 import numpy as np
 import pytest
@@ -23,29 +21,12 @@ if has_gpu():
     import torch
 
     import k8s_gpu_hpa_b200 as pkg
+    from gpu_helpers import (SIZES, assert_bits_equal, dev, geometry, k1d_tunes, profiled_kernel_name,
+                             trace_events)
     from k8s_gpu_hpa_b200 import capi, vector_add as va
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 ALL = ["auto", "k0", "k1", "k2", "k3"]
-SIZES = [0, 1, 2, 3, 4, 5, 7, 8, 9, 15, 16, 17, 31, 32, 33, 255, 256, 257, 1023, 4095, 4096, 4097,
-         50000, (1 << 16) - 1, (1 << 20) - 1, 1 << 20, (1 << 20) + 1, 3_000_017]
-
-
-def dev(x: np.ndarray):
-    return torch.from_numpy(np.ascontiguousarray(x)).cuda()
-
-
-def assert_bits_equal(got, want: np.ndarray, what=""):
-    g = got.cpu().numpy() if not isinstance(got, np.ndarray) else got
-    bad = oracle.first_mismatch(g, want)
-    assert bad < 0, f"{what}: first mismatch at {bad}: got {g.view(np.uint32)[bad]:08x} want {want.view(np.uint32)[bad]:08x}"
-
-
-def geometry(t, n, lib=None):
-    """b200va_geometry for tune t at n elements on the current device: (return code, grid, block)."""
-    grid, block = C.c_uint(), C.c_uint()
-    rc = (lib or capi.lib).b200va_geometry(C.byref(t), n, torch.cuda.current_device(), C.byref(grid), C.byref(block), None)
-    return rc, grid.value, block.value
 
 
 @pytest.mark.parametrize("variant", ALL)
@@ -235,12 +216,6 @@ def production_tunes():
             for flags in (0, capi.F_INPUTS_STABLE, capi.F_COLD, capi.F_COLD | capi.F_INPUTS_STABLE)]
 
 
-def k1d_tunes():
-    """The K1d (dynamic tile scheduler) tunes the production library carries."""
-    return (capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=2, st_hint=1, scheduler=1),
-            capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=4, st_hint=1, scheduler=1, early_loads=1))
-
-
 def test_production_library_carries_the_production_set_only():
     """libb200va.so: what AUTO and the named variants resolve to (+ early loads, + K1d) runs; a
     geometry only the A/B matrix has is refused with ERR_VARIANT -- and runs in libb200va_tune.so.
@@ -264,13 +239,6 @@ def test_production_library_carries_the_production_set_only():
     assert geometry(exotic, n, capi.tune_lib())[0] == capi.OK
 
 
-def _profiled_kernel_name(name: str) -> str:
-    """A kernel name as the profiler prints it, in Tune.kernel_name()'s form: no namespace, parameter list, casts
-    or spaces, and bools as 0/1."""
-    name = re.sub(r"\((?:int|bool|unsigned int)\)", "", name).replace("true", "1").replace("false", "0")
-    return re.match(r"(?:void )?(?:b200va::)?(\w+(?:<[^>]*>)?)", name).group(1).replace(" ", "")
-
-
 def test_launched_kernel_has_the_geometry_and_name_the_library_reports(tmp_path):
     """Every tune the production library resolves, and its K1d tunes, launched once under the profiler on
     256-byte-aligned buffers of the n it was resolved for: the kernel in the trace has b200va_geometry's grid and
@@ -292,11 +260,8 @@ def test_launched_kernel_has_the_geometry_and_name_the_library_reports(tmp_path)
             va.add(a[:n], b[:n], c[:n], tune=t)
             want.append((t.kernel_name(), grid, block, n))
         torch.cuda.synchronize()
-    trace = tmp_path / "trace.json"
-    prof.export_chrome_trace(str(trace))
-    events = sorted((e for e in json.loads(trace.read_text())["traceEvents"] if e.get("cat") == "kernel"),
-                    key=lambda e: e["ts"])
-    got = [(_profiled_kernel_name(e["name"]), e["args"]["grid"][0], e["args"]["block"][0]) for e in events]
+    events = trace_events(prof, tmp_path, ("kernel",))
+    got = [(profiled_kernel_name(e["name"]), e["args"]["grid"][0], e["args"]["block"][0]) for e in events]
     assert len(got) == len(want)
     for g, w in zip(got, want):
         assert g == w[:3], (g, w)

@@ -8,16 +8,7 @@ is the launch immediately before them on the stream.  Each case here is one chai
 
 and the tail's output is compared with the exact reference of its operation applied to the exact window.
 
-W is the production "k2" add (K2d, the TMA ring under the dynamic tile scheduler) at n = 2^28.  Its grid is
-persistent, one 544-thread CTA per SM with about 128 KiB of shared memory, so every CTA starts, and passes its
-trigger, at once; it then streams for about a millisecond, and the scheduler hands out tiles in order, so the end
-of X (where the window lies) is written last.  Each SM keeps about 1500 threads free, so the small middle and tail
-grids become resident beside it: a read of X that escapes the chain's order lands in a window about 1 ms wide and
-sees the poison.  A multi-wave writer would not do: its last wave passes the trigger only just before it ends.
-Nor would a K1d writer: its persistent grid fills the SMs, and nothing else becomes resident beside it.
-
-Middle launches fit beside W (about 2^16 elements).  k0, the mixed-phase stream op and fill_ctr are launched
-without the PDL attribute: they end the chain, and the cases behind them pass whatever the kernels do.
+gpu_helpers.py sets up W, the window and the middle launches, and says why they are chosen as they are.
 
 One run per case: the window is wide enough that one run decides it.  The same matrix runs once more in a
 subprocess with B200VA_NO_PDL=1 (the library reads it once per process), where every launch is an ordinary one.
@@ -29,98 +20,15 @@ import sys
 import numpy as np
 import pytest
 
-import oracle
 from conftest import ROOT, has_gpu
-from oracle import convert_exact as V
-from oracle import dot_exact as D
-from oracle import stream_exact as X
 
 pytestmark = pytest.mark.gpu
 if has_gpu():
     import torch
 
+    from gpu_helpers import LO, M, N, SCALE, _chains, _poison, _run
+    from gpu_helpers import env  # noqa: F401  (the module-scoped fixture)
     from k8s_gpu_hpa_b200 import capi, vector_add as va
-    from test_gpu_parity import k1d_tunes
-
-N = 1 << 28                        # W's length: the HBM class, about 1 ms of streaming on an H100
-LO = N - (1 << 18) - 3             # the window X[LO:LO + M]: ragged, 4 bytes past a 16-byte boundary
-M = (1 << 18) - 5
-SEED_P, SEED_Q, SEED_B = 0x0A, 0x0B, 0x0C
-POISON = 0x5A5A5A5A                # a finite f32 (about 1.5e16): a stale read gives a definite wrong value
-SMALL = 1 << 16                    # middle launches: grids that fit beside W
-SCALE = 3.0
-
-
-@pytest.fixture(scope="module")
-def env():
-    free, _ = torch.cuda.mem_get_info()
-    if free < (4 << 30):
-        pytest.skip(f"needs about 4 GiB of free device memory, {free >> 20} MiB free")
-    e = {}
-    e["P"] = va.fill_ctr(torch.empty(N, dtype=torch.float32, device="cuda"), SEED_P)
-    e["Q"] = va.fill_ctr(torch.empty(N, dtype=torch.float32, device="cuda"), SEED_Q)
-    e["X"] = torch.empty(N, dtype=torch.float32, device="cuda")
-    # tail operands and outputs share the window's 16-byte phase (one element past it), so the vector forms run
-    e["B"] = va.fill_ctr(torch.empty(M + 1, dtype=torch.float32, device="cuda"), SEED_B)[1:]
-    e["C"] = torch.empty(M + 1, dtype=torch.float32, device="cuda")[1:]
-    e["H"] = torch.empty(M + 1, dtype=torch.float16, device="cuda")[1:]
-    e["dot"] = torch.empty(1, dtype=torch.float64, device="cuda")
-    e["ws"] = torch.empty(max(capi.lib.b200va_dot_workspace_bytes(max(M, SMALL)), 8), dtype=torch.uint8, device="cuda")
-    # the middle launches' own buffers
-    e["ma"] = va.fill_ctr(torch.empty(SMALL + 4, dtype=torch.float32, device="cuda"), 0x1A)
-    e["mb"] = va.fill_ctr(torch.empty(SMALL + 4, dtype=torch.float32, device="cuda"), 0x1B)
-    e["mc"] = torch.empty(SMALL + 4, dtype=torch.float32, device="cuda")
-    e["mh"] = torch.empty(SMALL, dtype=torch.float16, device="cuda")
-    e["mdot"] = torch.empty(1, dtype=torch.float64, device="cuda")
-    torch.cuda.synchronize()
-    host_b = e["B"].cpu().numpy()
-    window = oracle.vadd(oracle.fill_ctr(M, SEED_P, LO), oracle.fill_ctr(M, SEED_Q, LO))
-    e["ref_window"] = window
-    e["ref_add"] = oracle.vadd(window, host_b)
-    e["ref_scale"] = X.stream("scale", "f32", window, None, SCALE)
-    e["ref_triad"] = X.stream("triad", "f32", window, host_b, SCALE)
-    e["ref_f16"] = V.convert(window, "f32", "f16")
-    e["ref_dot"] = D.dot(window, host_b, "f32")
-    yield e
-    del e
-    torch.cuda.empty_cache()
-
-
-# ------------------------------------------------------------------------------------------- middle launches
-def _middles(e):
-    """name -> (launch, launched with the PDL attribute)."""
-    a, b, c = e["ma"][:SMALL], e["mb"][:SMALL], e["mc"][:SMALL]
-    k1d = k1d_tunes()[0]
-    m = {
-        "add auto": (lambda: va.add(a, b, c), True),
-        "add k1": (lambda: va.add(a, b, c, variant="k1"), True),
-        "add k3": (lambda: va.add(a, b, c, variant="k3"), True),
-        "add k2 (K2d below the HBM class)": (lambda: va.add(a, b, c, variant="k2"), True),
-        "add k0": (lambda: va.add(a, b, c, variant="k0"), False),
-        "add K4 (mixed phase)": (lambda: va.add(e["ma"][:SMALL], e["mb"][1:SMALL + 1], e["mc"][2:SMALL + 2]), True),
-        "add K1d tune": (lambda: va.add(a, b, c, tune=k1d), True),
-        "stream copy": (lambda: va.stream("copy", a, out=c), True),
-        "stream scale": (lambda: va.stream("scale", a, out=c, scalar=SCALE), True),
-        "stream add": (lambda: va.stream("add", a, b, c), True),
-        "stream triad": (lambda: va.stream("triad", a, b, c, scalar=SCALE), True),
-        "stream add (mixed phase)": (lambda: va.stream("add", e["ma"][1:SMALL + 1], e["mb"][:SMALL], e["mc"][:SMALL]), False),
-        "convert f32->f16": (lambda: va.convert(a, "f16", e["mh"]), True),
-        "dot f32": (lambda: va.dot(a, b, out=e["mdot"], workspace=e["ws"]), True),
-        "probe copy": (lambda: va.probe("copy", a, None, c), True),
-        "fill_ctr": (lambda: va.fill_ctr(c, 0x1C), False),
-    }
-    return m
-
-
-def _chains(e):
-    """The middle sequences: none, each middle alone, and runs of two and three."""
-    m = _middles(e)
-    chains = [()] + [(k,) for k in m]
-    chains += [("add auto", "stream add"), ("convert f32->f16", "dot f32"), ("probe copy", "add K1d tune"),
-               ("add k2 (K2d below the HBM class)", "add k3"), ("stream triad", "add k0"),
-               ("add k1", "stream copy", "add auto"), ("dot f32", "add K4 (mixed phase)", "stream scale"),
-               ("fill_ctr", "add auto", "add k1"), ("add auto", "add k0", "stream add")]
-    return m, chains
 
 
 # ------------------------------------------------------------------------------------------- tails
@@ -168,23 +76,6 @@ def _tails(e):
         "convert f32->f16": (lambda w: va.convert(w, "f16", H), f16_ok, False),
         "dot f32": (lambda w: va.dot(w, B, out=e["dot"], workspace=e["ws"]), dot_ok, False),
     }
-
-
-def _poison(e):
-    e["X"].view(torch.int32).fill_(POISON)
-    e["C"].fill_(-7.0)
-    e["H"].fill_(-7.0)
-    e["dot"].fill_(-7.0)
-
-
-def _run(e, middles, names, tail):
-    """One chain on the current stream, one synchronise: the tail's output is left for its check."""
-    _poison(e)
-    va.add(e["P"], e["Q"], e["X"], variant="k2")
-    for k in names:
-        middles[k][0]()
-    tail(e["X"][LO:LO + M])
-    torch.cuda.synchronize()
 
 
 def test_early_load_sizes_resolve_to_register_loads_ahead_of_the_wait():

@@ -16,7 +16,6 @@ matches NaN as a class).  Outputs are poisoned beforehand and guard elements on 
 This module's name sorts after test_gpu_parity.py and test_gpu_stream.py, whose traces lose kernels behind a module
 with profiler traces that runs before them (DESIGN.md section 3).
 """
-import json
 import math
 
 import numpy as np
@@ -32,18 +31,13 @@ pytestmark = pytest.mark.gpu
 if has_gpu():
     import torch
 
+    from gpu_helpers import (ES, GUARD, INT, LO, POISON, TORCH, M, _chains, _run, assert_guards, assert_matches,
+                             expected_cast_launch, kernels_after_marker, poisoned, tiled, to_dev)
+    from gpu_helpers import env  # noqa: F401  (the module-scoped fixture)
     from k8s_gpu_hpa_b200 import capi, vector_add as va
-    from test_gpu_parity import _profiled_kernel_name
-    from test_gpu_pdl_chains import LO, M, _chains, _run, env  # noqa: F401  (env: the module-scoped fixture)
-    from test_gpu_stream import GUARD, POISON, assert_guards, assert_matches, tiled, to_dev
-    from test_gpu_typecast import expected_cast_launch
-
-    TORCH = {"f16": torch.float16, "bf16": torch.bfloat16, "e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
-    INT = {"f16": torch.int16, "bf16": torch.int16, "e4m3": torch.uint8, "e5m2": torch.uint8}
 
 DESTS = S.DESTS
 FP8 = ("e4m3", "e5m2")
-ESC = {"f16": 2, "bf16": 2, "e4m3": 1, "e5m2": 1}
 G = {"f16": 8, "bf16": 8, "e4m3": 16, "e5m2": 16}
 SEED = 0x5EED
 PERIOD = 199_999
@@ -68,44 +62,12 @@ def sr(a, dst, out, seed=SEED, first=0, k=0, **kw):
     return va.convert_sr(a, TORCH[dst], seed=seed, offset=first, out=out, **kw)
 
 
-def bits_dev(x: np.ndarray, dst: str):
-    t = torch.from_numpy(np.ascontiguousarray(x)).cuda()
-    return t.view(TORCH[dst])
-
-
-def poisoned_out(n, dst, off=0):
-    buf = torch.empty((GUARD + off + n + GUARD) * ESC[dst], dtype=torch.uint8, device="cuda")
-    buf.fill_(POISON)
-    return buf.view(TORCH[dst]), buf.view(TORCH[dst])[GUARD + off:GUARD + off + n]
-
-
-def _nan(t, dst):
-    u = t.view(INT[dst]).to(torch.int32)
-    if dst == "e4m3":
-        return (u & 0x7F) == 0x7F
-    if dst == "e5m2":
-        return (u & 0x7F) > 0x7C
-    return (u & 0x7FFF) > (0x7C00 if dst == "f16" else 0x7F80)
-
-
-def assert_same(got, want, dst, what="", chunk=1 << 28):
-    """Bit patterns equal element by element on the device, NaN matching NaN as a class."""
-    assert got.numel() == want.numel(), what
-    for lo in range(0, got.numel(), chunk):
-        g, w = got[lo:lo + chunk], want[lo:lo + chunk]
-        bad = (g.view(INT[dst]) != w.view(INT[dst])) & ~(_nan(g, dst) & _nan(w, dst))
-        if bool(bad.any()):
-            i = int(torch.nonzero(bad)[0])
-            raise AssertionError(f"{what}: {int(bad.sum())} mismatches, first at {lo + i} of {got.numel()}: "
-                                 f"got {int(g.view(INT[dst])[i])} want {int(w.view(INT[dst])[i])} (bits)")
-
-
 def check(a_host, a_dev, dst, seed, first, k=0, off_c=0, what=""):
     n = a_host.size
-    buf, out = poisoned_out(n, dst, off_c)
+    buf, out = poisoned(n, dst, off_c)
     sr(a_dev, dst, out, seed, first, k)
     torch.cuda.synchronize()
-    assert_same(out, bits_dev(oracle_sr(a_host, dst, seed, first, k), dst), dst, what)
+    assert_matches(out, to_dev(oracle_sr(a_host, dst, seed, first, k), dst), dst, what)
     assert_guards(buf, GUARD + off_c, n, what)
 
 
@@ -130,13 +92,13 @@ def test_sizes_around_the_group_at_every_offset(dst):
     for first in (0, 1, (1 << 32) + 5):
         for oa in range(4):
             want_all = oracle_sr(host[oa:oa + max(sizes)], dst, SEED, first, k)
-            for oc in range(16 // ESC[dst]):
+            for oc in range(16 // ES[dst]):
                 for n in sizes:
                     a, what = abuf[GUARD + oa:GUARD + oa + n], f"{dst} n={n} first={first} offsets A {oa} C {oc}"
-                    buf, out = poisoned_out(n, dst, oc)
+                    buf, out = poisoned(n, dst, oc)
                     sr(a, dst, out, SEED, first, k)
                     torch.cuda.synchronize()
-                    assert_same(out, bits_dev(want_all[:n], dst), dst, what)
+                    assert_matches(out, to_dev(want_all[:n], dst), dst, what)
                     assert_guards(buf, GUARD + oc, n, what)
 
 
@@ -190,13 +152,13 @@ def test_both_sides_of_the_hbm_edge(dst):
     a = tiled(block, big + 1, "f32")
     k = k_of(dst)
     first = 12345
-    want = bits_dev(oracle_sr(host, dst, SEED, first, k), dst)        # element i of A has the global index first + i
+    want = to_dev(oracle_sr(host, dst, SEED, first, k), dst)          # element i of A has the global index first + i
     for n, off in ((h - 1, 0), (h, 0), (big, 1)):
         what = f"{dst} n={n} offset {off}"
-        buf, out = poisoned_out(n, dst, off)
+        buf, out = poisoned(n, dst, off)
         sr(a[off:off + n], dst, out, SEED, first + off, k)
         torch.cuda.synchronize()
-        assert_same(out, want[off:off + n], dst, what)
+        assert_matches(out, want[off:off + n], dst, what)
         assert_guards(buf, GUARD + off, n, what)
         del buf, out
 
@@ -208,25 +170,25 @@ def test_beyond_32_bit_offsets_with_first_near_2_40(dst):
     n = (1 << 32) + 4099
     torch.cuda.empty_cache()
     free, _ = torch.cuda.mem_get_info()
-    if free < 4 * n + 3 * ESC[dst] * n + (4 << 30):
+    if free < 4 * n + 3 * ES[dst] * n + (4 << 30):
         pytest.skip("needs ~45 GiB of free device memory")
     first = (1 << 40) - 3
     k = k_of(dst)
     block = random_f32(PERIOD, np.random.default_rng(31))
     a = tiled(block, n, "f32")
-    c = torch.empty(n * ESC[dst], dtype=torch.uint8, device="cuda").view(TORCH[dst])
+    c = torch.empty(n * ES[dst], dtype=torch.uint8, device="cuda").view(TORCH[dst])
     sr(a, dst, c, SEED, first, k)
     for lo in ((1 << 31) - 4096, (1 << 32) - 4096, n - 8192):
         x = np.tile(block, 2 * (8192 // PERIOD + 2))
         start = lo % PERIOD
         win = x[start:start + 8192]
-        assert_same(c[lo:lo + 8192], bits_dev(oracle_sr(win, dst, SEED, first + lo, k), dst), dst, f"window at {lo}")
+        assert_matches(c[lo:lo + 8192], to_dev(oracle_sr(win, dst, SEED, first + lo, k), dst), dst, f"window at {lo}")
     m = (1 << 32) - 77
     parts = torch.empty_like(c)
     sr(a[:m], dst, parts[:m], SEED, first, k)
     sr(a[m:], dst, parts[m:], SEED, first + m, k)
     torch.cuda.synchronize()
-    assert_same(parts, c, dst, "two calls against one, n = 2^32 + 4099")
+    assert_matches(parts, c, dst, "two calls against one, n = 2^32 + 4099")
 
 
 # ------------------------------------------------------------------------------------------- reproducibility
@@ -237,15 +199,15 @@ def test_two_calls_equal_one_call(dst):
     a = to_dev(host, "f32")
     k = k_of(dst)
     for first in (0, 3, (1 << 64) - 1000, (1 << 64) - 1003):        # groups of 16 and of 8 across 2^64
-        whole = torch.empty(n * ESC[dst], dtype=torch.uint8, device="cuda").view(TORCH[dst])
+        whole = torch.empty(n * ES[dst], dtype=torch.uint8, device="cuda").view(TORCH[dst])
         sr(a, dst, whole, SEED, first, k)
-        assert_same(whole, bits_dev(oracle_sr(host, dst, SEED, first, k), dst), dst, f"{dst} first {first}")
+        assert_matches(whole, to_dev(oracle_sr(host, dst, SEED, first, k), dst), dst, f"{dst} first {first}")
         for m in (1, 5, G[dst], 1001, n - 3):
             parts = torch.empty_like(whole)
             sr(a[:m], dst, parts[:m], SEED, first, k)
             sr(a[m:], dst, parts[m:], SEED, (first + m) % (1 << 64), k)
             torch.cuda.synchronize()
-            assert_same(parts, whole, dst, f"{dst} first {first} split at {m}")
+            assert_matches(parts, whole, dst, f"{dst} first {first} split at {m}")
 
 
 def test_repeats_and_graph_replays_give_the_same_bytes_and_another_seed_differs():
@@ -253,14 +215,14 @@ def test_repeats_and_graph_replays_give_the_same_bytes_and_another_seed_differs(
     rng = np.random.default_rng(7)
     host = (rng.standard_normal(n) * 300).astype(np.float32)
     a = to_dev(host, "f32")
-    outs = {d: poisoned_out(n, d, 1) for d in DESTS}
+    outs = {d: poisoned(n, d, 1) for d in DESTS}
     amax = torch.zeros(1, dtype=torch.float64, device="cuda")
-    wants = {d: bits_dev(oracle_sr(host, d, SEED, 11, k_of(d)), d) for d in DESTS}
+    wants = {d: to_dev(oracle_sr(host, d, SEED, 11, k_of(d)), d) for d in DESTS}
     for d in DESTS:
         for _ in range(2):
             sr(a, d, outs[d][1], SEED, 11, k_of(d))
             torch.cuda.synchronize()
-            assert_same(outs[d][1], wants[d], d, f"{d} repeated")
+            assert_matches(outs[d][1], wants[d], d, f"{d} repeated")
         other = torch.empty_like(outs[d][1])
         sr(a, d, other, SEED + 1, 11, k_of(d))
         torch.cuda.synchronize()
@@ -283,7 +245,7 @@ def test_repeats_and_graph_replays_give_the_same_bytes_and_another_seed_differs(
         g.replay()
         torch.cuda.synchronize()
         for d in DESTS:
-            assert_same(outs[d][1], wants[d], d, f"{d} graph replay {r}")
+            assert_matches(outs[d][1], wants[d], d, f"{d} graph replay {r}")
             assert_guards(outs[d][0], GUARD + 1, n, f"{d} graph replay {r}")
         assert float(amax.item()) == F.amax(host, "f32")
 
@@ -306,7 +268,7 @@ def test_amax_equals_quantize_fp8s():
             got, want = float(m_sr.item()), float(m_rn.item())
             assert (math.isnan(got) and math.isnan(want)) or \
                 np.float64(got).view(np.uint64) == np.float64(want).view(np.uint64), (name, fmt, got, want)
-            assert_same(q, bits_dev(oracle_sr(x, fmt, 1, 0, 4), fmt), fmt, f"{name} {fmt}")
+            assert_matches(q, to_dev(oracle_sr(x, fmt, 1, 0, 4), fmt), fmt, f"{name} {fmt}")
 
 
 # ------------------------------------------------------------------------------------------- arguments
@@ -431,34 +393,21 @@ def test_trace_shows_the_planned_kernel(tmp_path):
     profiler the kernels after the marker are exactly the planned ones with their grid and block."""
     h = 1 << 25
     src = torch.zeros(h + 64, dtype=torch.float32, device="cuda")
-    outs = {d: torch.zeros((h + 64) * ESC[d], dtype=torch.uint8, device="cuda").view(TORCH[d]) for d in DESTS}
+    outs = {d: torch.zeros((h + 64) * ES[d], dtype=torch.uint8, device="cuda").view(TORCH[d]) for d in DESTS}
     plan, want = [], []
     for d in DESTS:
         for n, oa, oc in ((1000, 0, 0), (h, 0, 0), (1001, 0, 1), (4099, 1, 1)):
             a, c = src[oa:oa + n], outs[d][oc:oc + n]
             plan.append((d, a, c))
-            want.append(expected_cast_launch("sr_cast_vec", 4, ESC[d], n, a.data_ptr(), c.data_ptr()))
-    marker = torch.zeros(1, device="cuda")
+            want.append(expected_cast_launch("sr_cast_vec", 4, ES[d], n, a.data_ptr(), c.data_ptr()))
     amax = torch.zeros(1, dtype=torch.float64, device="cuda")
-    torch.cuda.synchronize()
 
     def run_plan():
         for d, a, c in plan:
             sr(a, d, c, SEED, 0, k_of(d), **({"amax": amax} if d in FP8 else {}))
         torch.cuda.synchronize()
 
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        run_plan()
-        marker.fill_(1.0)
-        torch.cuda.synchronize()
-        run_plan()
-    trace = tmp_path / "trace.json"
-    prof.export_chrome_trace(str(trace))
-    events = sorted((e for e in json.loads(trace.read_text())["traceEvents"] if e.get("cat") in ("kernel", "gpu_memset")),
-                    key=lambda e: e["ts"])
-    mk = max(i for i, e in enumerate(events) if "sr_cast_vec" not in e["name"])
-    assert events[mk].get("cat") == "kernel" and "ill" in events[mk]["name"], events[mk]["name"]
-    got = [(_profiled_kernel_name(e["name"]), e["args"]["grid"][0], e["args"]["block"][0]) for e in events[mk + 1:]]
+    got = kernels_after_marker(tmp_path, run_plan, ("sr_cast_vec",))
     assert len(got) == len(want), (len(got), len(want), got[:8])
     for g, w, p in zip(got, want, plan):
         assert g == w, (p[0], g, w)

@@ -18,13 +18,13 @@ import pytest
 
 import oracle
 from conftest import has_gpu
-from test_gpu_parity import SIZES, assert_bits_equal, dev
 
 pytestmark = pytest.mark.gpu
 if has_gpu():
     import torch
 
     import k8s_gpu_hpa_b200 as pkg
+    from gpu_helpers import SIZES, assert_bits_equal, dev
     from k8s_gpu_hpa_b200 import capi, vector_add as va
 
 RING = 4096                 # ticket-counter slots per device (kSchedSlots)

@@ -13,8 +13,8 @@ pytestmark = pytest.mark.gpu
 if has_gpu():
     import torch
 
+    from gpu_helpers import geometry, profiled_kernel_name
     from k8s_gpu_hpa_b200 import capi, vector_add as va
-    from test_gpu_parity import _profiled_kernel_name, geometry
 
 MODES = [0, 2, 3, 4]        # slot streams, lanes, pageable bounce ring, register-once
 CASES = [                   # (n, chunk, depth)
@@ -109,7 +109,7 @@ def test_stager_trace_follows_the_chunk_schedule(tmp_path, marker, mode, n, chun
         t = capi.resolve(capi.K_AUTO, mk, capi.F_COLD)
         rc, grid, block = geometry(t, mk)
         assert rc == capi.OK
-        assert (_profiled_kernel_name(kern["name"]), kern["args"]["grid"][0], kern["args"]["block"][0]) == \
+        assert (profiled_kernel_name(kern["name"]), kern["args"]["grid"][0], kern["args"]["block"][0]) == \
                (t.kernel_name(), grid, block), (k, mk)
         # data flow: the add reads what the H2D copies wrote, the D2H copy reads what the add wrote
         assert start(kern) >= max(end(a), end(b)), k

@@ -11,14 +11,13 @@ Large inputs repeat a random block of PERIOD elements (odd, so it never lines up
 reference of an elementwise op is then the block's reference repeated, exact at every element for little host work.
 Outputs are filled with a finite byte pattern beforehand, and guard elements on both sides must keep it.
 """
-import json
 import re
-import subprocess
 
 import numpy as np
 import pytest
 
 import oracle
+import sass
 from conftest import has_gpu
 from oracle import stream_exact as X
 
@@ -27,22 +26,16 @@ if has_gpu():
     import torch
 
     import k8s_gpu_hpa_b200 as pkg
+    from gpu_helpers import (DT_CODE, ES, GUARD, POISON, TORCH, assert_guards, assert_matches, kernels_after_marker,
+                             poisoned, tiled, to_dev)
     from k8s_gpu_hpa_b200 import capi, vector_add as va
-    from test_gpu_parity import _profiled_kernel_name
-
-    TORCH = {"f32": torch.float32, "f64": torch.float64, "f16": torch.float16, "bf16": torch.bfloat16}
-    INT = {"f32": torch.int32, "f64": torch.int64, "f16": torch.int16, "bf16": torch.int16}
 
 OPS = ["copy", "scale", "add", "triad"]
 DTS = ["f32", "f64", "f16", "bf16"]
 SIZES = [0, 1, 2, 3, 7, 8, 9, 15, 16, 17, 1023, 4097, 50000, (1 << 20) + 3, 5_000_011]
-ES = {"f32": 4, "f64": 8, "f16": 2, "bf16": 2}
-DT_CODE = {"f32": 0, "f64": 1, "f16": 2, "bf16": 3}
 OP_CODE = {"copy": 0, "scale": 1, "add": 2, "triad": 3}
 BINARY = ("add", "triad")
 PERIOD = 199_999            # <= X.FRACTION_LIMIT: f64 TRIAD is exact through Fraction over a whole period
-POISON = 0x5A               # byte fill: finite in every type (f16 0x5A5A = 203.25, bf16 1.5e16, f32 1.5e16, f64 ~4e127)
-GUARD = 8                   # guard elements on each side; 8 elements keep the first element 16-byte aligned
 SCALARS = [0.1, 1 / 3, 1 + 2.0 ** -24, 1 + 2.0 ** -24 + 2.0 ** -52, 3.5e38, 1e-45, 1e-50, -0.0,
            float("inf"), float("-inf"), float("nan")]
 
@@ -58,54 +51,10 @@ def host_inputs(dtype, n, seed):
             rng.integers(0, 1 << 16, n, dtype=np.uint32).astype(np.uint16))
 
 
-def to_dev(x, dtype):
-    t = torch.from_numpy(np.ascontiguousarray(x)).cuda()
-    if dtype == "f16":
-        return t.view(torch.float16)
-    if dtype == "bf16":
-        return t.view(torch.bfloat16)
-    return t
-
-
 def to_host(t, dtype):
     if dtype in ("f16", "bf16"):
         return t.view(torch.int16).cpu().numpy().view(np.uint16)
     return t.cpu().numpy()
-
-
-def poisoned(n, dtype, off=0):
-    """(buffer, view): GUARD + off + n + GUARD elements of POISON bytes, the view is the n after GUARD + off."""
-    buf = torch.empty(GUARD + off + n + GUARD, dtype=TORCH[dtype], device="cuda")
-    buf.view(torch.uint8).fill_(POISON)
-    return buf, buf[GUARD + off:GUARD + off + n]
-
-
-def assert_guards(buf, start, n, what=""):
-    """The GUARD elements before `start` and after start + n in buf still hold the poison."""
-    es = buf.element_size()
-    u8 = buf.view(torch.uint8)
-    lo, hi = u8[max(0, start - GUARD) * es:start * es], u8[(start + n) * es:(start + n + GUARD) * es]
-    assert bool((lo == POISON).all()) and bool((hi == POISON).all()), f"{what}: a guard element was written"
-
-
-def assert_matches(got, want, dtype, what="", nan_class=True, chunk=1 << 28):
-    """Element by element on the device: the bit patterns are equal (NaN matches NaN as a class if nan_class)."""
-    assert got.numel() == want.numel()
-    for lo in range(0, got.numel(), chunk):
-        g, w = got[lo:lo + chunk], want[lo:lo + chunk]
-        bad = g.view(INT[dtype]) != w.view(INT[dtype])
-        if nan_class:
-            bad &= ~(torch.isnan(g) & torch.isnan(w))
-        if bool(bad.any()):
-            i = int(torch.nonzero(bad)[0])
-            raise AssertionError(f"{what}: {int(bad.sum())} mismatches, first at {lo + i} of {got.numel()}: "
-                                 f"got {int(g.view(INT[dtype])[i])} want {int(w.view(INT[dtype])[i])} (bits)")
-
-
-def tiled(x, n, dtype):
-    """A device tensor of n elements: the host block x repeated."""
-    t = to_dev(x, dtype)
-    return t.repeat(-(-n // t.numel()))[:n] if n > t.numel() else t[:n].contiguous()
 
 
 def run(op, a, b, c, s=0.0, stream=None):
@@ -249,15 +198,18 @@ def test_every_size_class_and_both_sides_of_each_edge(op, dtype):
 
 def library_stream_kernels(path):
     """stream_* kernels in a library, as the profiler names them: stream_vec<DT,OP,UNROLL,LD,ST>, stream_scalar<DT,OP>."""
-    out = subprocess.run(["cuobjdump", "-symbols", path], capture_output=True, text=True, check=True).stdout
-    return {f"{k}<{','.join(re.findall(r'Li(-?\d+)E', args))}>"
-            for k, args in re.findall(r"_ZN6b200va\d+(stream_vec|stream_scalar)I((?:Li-?\d+E)+)E", out)}
+    out = set()
+    for fn in sass.functions(path):
+        m = re.match(r"_ZN6b200va\d+(stream_vec|stream_scalar)I((?:Li-?\d+E)+)E", fn)
+        if m:
+            out.add(f"{m[1]}<{','.join(re.findall(r'Li(-?\d+)E', m[2]))}>")
+    return out
 
 
 def test_every_stream_kernel_of_the_library_is_launched_with_the_dispatchers_geometry(tmp_path):
     """One launch per dtype, op and size class, plus one through the mixed-misalignment scalar path, under the
     profiler: each kernel's template arguments, grid and block are the table's in launch_stream_typed, and the
-    kernels launched are exactly the stream kernels cuobjdump lists for libb200va.so.  prefetch_first is a runtime
+    kernels launched are exactly the stream kernels in the SASS of libb200va.so.  prefetch_first is a runtime
     argument the trace cannot show; the dispatcher sets it under the m >= 2^25 condition that picks the ST_NA
     (store hint 1) kernels, so a launched ST_NA kernel ran the prefetch."""
     plan, want = [], []
@@ -273,8 +225,6 @@ def test_every_stream_kernel_of_the_library_is_launched_with_the_dispatchers_geo
     for dtype in DTS:
         nmax = max(n for _, d, n, _ in plan if d == dtype) + 1
         bufs[dtype] = [torch.zeros(nmax, dtype=TORCH[dtype], device="cuda") for _ in range(3)]
-    marker = torch.zeros(1, device="cuda")
-    torch.cuda.synchronize()
 
     def run_plan():
         for op, dtype, n, off in plan:
@@ -282,21 +232,7 @@ def test_every_stream_kernel_of_the_library_is_launched_with_the_dispatchers_geo
             run(op, a[off:off + n], b[off:off + n], c[:n], 0.5)
         torch.cuda.synchronize()
 
-    # As in test_gpu_stream_dot.py: the trace can miss the first kernels after the profiler starts (three warm-up
-    # kernels and the plan's first launch, seen once).  So the plan runs twice, a fill kernel marks the start of the
-    # second pass, and the second pass is checked.
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        run_plan()
-        marker.fill_(1.0)
-        torch.cuda.synchronize()
-        run_plan()
-    trace = tmp_path / "trace.json"
-    prof.export_chrome_trace(str(trace))
-    events = sorted((e for e in json.loads(trace.read_text())["traceEvents"] if e.get("cat") in ("kernel", "gpu_memset")),
-                    key=lambda e: e["ts"])
-    m = max(i for i, e in enumerate(events) if "stream_" not in e["name"])   # the marker: only stream kernels after it
-    assert events[m].get("cat") == "kernel" and "ill" in events[m]["name"], events[m]["name"]
-    got = [(_profiled_kernel_name(e["name"]), e["args"]["grid"][0], e["args"]["block"][0]) for e in events[m + 1:]]
+    got = kernels_after_marker(tmp_path, run_plan, ("stream_",))
     assert len(got) == len(want), (len(got), len(want), got[:8])
     for g, w, p in zip(got, want, plan):
         assert g == w, (p, g, w)

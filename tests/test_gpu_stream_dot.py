@@ -10,7 +10,6 @@
 - Argument errors, and nothing written outside d_out and the workspace bytes the call needs.
 - A profiler trace of the launches: exactly the planned kernels with their grid and block, and nothing else.
 """
-import json
 import math
 
 import numpy as np
@@ -24,28 +23,13 @@ pytestmark = pytest.mark.gpu
 if has_gpu():
     import torch
 
+    from gpu_helpers import DT_CODE, ES, POISON, TORCH, hbm_n, kernels_after_marker, to_dev
     from k8s_gpu_hpa_b200 import capi, vector_add as va
-    from test_gpu_parity import _profiled_kernel_name
-
-    TORCH = {"f32": torch.float32, "f64": torch.float64, "f16": torch.float16, "bf16": torch.bfloat16}
 
 DTS = ["f32", "f64", "f16", "bf16"]
-ES = {"f32": 4, "f64": 8, "f16": 2, "bf16": 2}
-DT_CODE = {"f32": 0, "f64": 1, "f16": 2, "bf16": 3}
 FORM = {"f32": (512, 4), "f64": (512, 2), "f16": (256, 4), "bf16": (256, 4)}     # dot_form: threads, rows
 SMALL = [0, 1, 2, 3, 7, 8, 9, 15, 16, 17, D.LANES - 1, D.LANES + 1, D.CHUNK - 1, D.CHUNK + 1, 2 * D.CHUNK + 3,
          5_000_011]
-POISON = 0x5A
-
-
-def to_dev(x, dtype):
-    t = torch.from_numpy(np.ascontiguousarray(x)).cuda()
-    return t.view(TORCH[dtype]) if dtype in ("f16", "bf16") else t
-
-
-def hbm_n(dtype):
-    """The smallest n in the HBM class: n * sizeof(T) / 4 >= 2^25."""
-    return (1 << 25) * 4 // ES[dtype]
 
 
 def bits(x: float) -> int:
@@ -75,7 +59,7 @@ def inputs(dtype, n, seed):
 
 @pytest.mark.parametrize("dtype", DTS)
 def test_sizes_and_both_sides_of_the_hbm_class(dtype):
-    h = hbm_n(dtype)
+    h = hbm_n(ES[dtype])
     ragged = h + 5 * D.CHUNK + 1234                   # 2^25 words + 5 chunks: a chunk count that is no power of two
     for n in SMALL + [h - 1, h, ragged]:
         a, b, want = inputs(dtype, n, n)
@@ -188,7 +172,7 @@ def test_small_dot_reading_the_end_of_a_large_stream_op(dtype):
     """A large HBM-class stream op writes C, and a one-chunk dot right behind it reads the last elements of C,
     which the large launch's last CTAs write last: only the dot's wait keeps it from loading stale values.  Ten
     pairs with a different scalar each, so a stale load finds the previous pair's values."""
-    n = hbm_n(dtype) + 5
+    n = hbm_n(ES[dtype]) + 5
     m = D.CHUNK - 3
     rng = np.random.default_rng(31)
     pa, pb = X.finite(dtype, 49_999, rng, 1.0), X.finite(dtype, m, rng, 1.0)
@@ -304,10 +288,10 @@ def test_trace_shows_exactly_the_planned_kernels(tmp_path):
 
     bufs = {}
     for dtype in DTS:
-        nmax = hbm_n(dtype) + 64
-        bufs[dtype] = (torch.zeros(nmax, dtype=TORCH[dtype], device="cuda"), torch.zeros(nmax, dtype=TORCH[dtype], device="cuda"))
+        h = hbm_n(ES[dtype])
+        bufs[dtype] = (torch.zeros(h + 64, dtype=TORCH[dtype], device="cuda"), torch.zeros(h + 64, dtype=TORCH[dtype], device="cuda"))
         threads, rows = FORM[dtype]
-        for n, off in ((0, 0), (1000, 0), (3 * D.CHUNK + 5, 0), (hbm_n(dtype), 0), (hbm_n(dtype) - 1, 0), (5000, 1)):
+        for n, off in ((0, 0), (1000, 0), (3 * D.CHUNK + 5, 0), (h, 0), (h - 1, 0), (5000, 1)):
             k = -(-n // D.CHUNK)
             plan.append((dtype, n, off))
             if n and off:
@@ -321,8 +305,6 @@ def test_trace_shows_exactly_the_planned_kernels(tmp_path):
     want += [("dot_vec<2,256,4>", 8194, 256)] + final(8194)
     out = torch.empty(1, dtype=torch.float64, device="cuda")
     ws = torch.empty(capi.lib.b200va_dot_workspace_bytes(big_n), dtype=torch.uint8, device="cuda")
-    marker = torch.zeros(1, device="cuda")
-    torch.cuda.synchronize()
 
     def run_plan():
         for dtype, n, off in plan:
@@ -333,20 +315,7 @@ def test_trace_shows_exactly_the_planned_kernels(tmp_path):
                 va.dot(a[:n], b[off:off + n], out=out, workspace=ws)
         torch.cuda.synchronize()
 
-    # Late in a long test session the trace can miss the first kernels after the profiler starts.  So the plan
-    # runs twice, a fill kernel marks the start of the second pass, and the second pass is checked.
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        run_plan()
-        marker.fill_(1.0)
-        torch.cuda.synchronize()
-        run_plan()
-    trace = tmp_path / "trace.json"
-    prof.export_chrome_trace(str(trace))
-    events = sorted((e for e in json.loads(trace.read_text())["traceEvents"] if e.get("cat") in ("kernel", "gpu_memset")),
-                    key=lambda e: e["ts"])
-    m = max(i for i, e in enumerate(events) if "dot_" not in e["name"])   # the marker: nothing but dot kernels after it
-    assert events[m].get("cat") == "kernel" and "ill" in events[m]["name"], events[m]["name"]
-    got = [(_profiled_kernel_name(e["name"]), e["args"]["grid"][0], e["args"]["block"][0]) for e in events[m + 1:]]
+    got = kernels_after_marker(tmp_path, run_plan, ("dot_",))
     assert len(got) == len(want), (len(got), len(want), got[:8])
     for g, w in zip(got, want):
         assert g == w, (g, w)

@@ -15,8 +15,6 @@ must keep the poison.
 This module's name sorts after test_gpu_stream_dot.py: a module with profiler traces that runs before the parity
 and stream modules makes their traces lose kernels (DESIGN.md section 3).
 """
-import json
-
 import numpy as np
 import pytest
 
@@ -28,25 +26,16 @@ pytestmark = pytest.mark.gpu
 if has_gpu():
     import torch
 
+    from gpu_helpers import (DT_CODE, ES, GUARD, POISON, TORCH, assert_guards, assert_matches, expected_cast_launch,
+                             hbm_n, kernels_after_marker, poisoned, tiled, to_dev)
     from k8s_gpu_hpa_b200 import capi, vector_add as va
-    from test_gpu_parity import _profiled_kernel_name
-    from test_gpu_stream import GUARD, POISON, assert_guards, assert_matches, poisoned, tiled, to_dev
-
-    TORCH = {"f32": torch.float32, "f64": torch.float64, "f16": torch.float16, "bf16": torch.bfloat16}
 
 PAIRS = V.PAIRS
-ES = V.SIZE
-DT_CODE = {"f32": 0, "f64": 1, "f16": 2, "bf16": 3}
 PERIOD = 199_999
 
 
 def group(src, dst):
     return 16 // min(ES[src], ES[dst])
-
-
-def hbm_n(src, dst):
-    """The smallest n in the HBM class: the wider operand holds at least 2^25 four-byte words."""
-    return (1 << 25) * 4 // max(ES[src], ES[dst])
 
 
 def convert(a, dst, out, **kw):
@@ -116,7 +105,7 @@ def test_the_low_parts_that_decide_the_rounding(src, dst):
 def test_both_sides_of_the_hbm_edge(src, dst):
     """n = h - 1 and h at aligned pointers, then h + 37 with A and C one element past a 16-byte boundary: the
     vector body with a head, in the HBM class (L2 prefetch ahead of the wait, no-allocate stores)."""
-    h = hbm_n(src, dst)
+    h = hbm_n(max(ES[src], ES[dst]))
     big = h + 37
     block = V.random_bits(src, PERIOD, np.random.default_rng([7, DT_CODE[src], DT_CODE[dst]]))
     a, want = tiled(block, big + 1, src), tiled(V.convert(block, src, dst), big + 1, dst)
@@ -204,7 +193,7 @@ def test_stream_op_convert_stream_op_on_one_stream():
         for s in scalars:
             c = V.convert(X.stream("scale", src, a0, None, s), src, dst)
             wants.append(X.stream("scale", dst, c, None, 0.5))
-        for n in ((1 << 20) + 5, hbm_n(src, dst) + 5):
+        for n in ((1 << 20) + 5, hbm_n(max(ES[src], ES[dst])) + 5):
             a = tiled(a0, n, src)
             b = torch.empty_like(a)
             c = torch.empty(n, dtype=TORCH[dst], device="cuda")
@@ -266,34 +255,16 @@ def test_f16_to_bf16_beyond_32_bit_offsets():
     assert_matches(c, want, "bf16", "n = 2^32 + 4099")
 
 
-def expected_cast_launch(kernel, esa, esc, n, a_ptr, c_ptr, units_per_group=1):
-    """(kernel, grid, block) of plan_cast (b200va_typed.cu): n elements of esa bytes at a_ptr cast to esc bytes at
-    c_ptr, with units_per_group units of work per group."""
-    G = 16 // min(esa, esc)
-    head, h = n, ((16 - a_ptr % 16) % 16) // esa
-    while h < G:
-        if (c_ptr + h * esc) % 16 == 0:
-            head = h
-            break
-        h += 16 // esa
-    head = min(head, n)
-    ngroups = (n - head) // G
-    units = ngroups * units_per_group
-    edges = n - ngroups * G
-    threads, unroll = (512, 2) if n >= (1 << 25) * 4 // max(esa, esc) else (256, 1)
-    blocks = max(-(-units // (threads * unroll)), -(-edges // threads))
-    return kernel, max(1, min(blocks, 2 ** 31 - 1)), threads
-
-
 def test_trace_shows_the_planned_kernels(tmp_path):
     """Per pair: n = 1000, the HBM class, n = 1001 in mixed phase, and an odd n with a head; per type the same-type
     call, which is the COPY stream kernel.  Under the profiler the kernels after the marker are exactly the
     planned ones with their grid and block."""
-    bufs = {dt: torch.zeros(max(hbm_n(s, d) for s, d in PAIRS) + 64, dtype=TORCH[dt], device="cuda") for dt in V.DTYPES}
+    nmax = max(hbm_n(max(ES[s], ES[d])) for s, d in PAIRS) + 64
+    bufs = {dt: torch.zeros(nmax, dtype=TORCH[dt], device="cuda") for dt in V.DTYPES}
     outs = {dt: torch.zeros_like(bufs[dt]) for dt in V.DTYPES}
     plan, want = [], []
     for src, dst in PAIRS:
-        for n, oa, oc in ((1000, 0, 0), (hbm_n(src, dst), 0, 0), (1001, 0, 1), (4099, 1, 1)):
+        for n, oa, oc in ((1000, 0, 0), (hbm_n(max(ES[src], ES[dst])), 0, 0), (1001, 0, 1), (4099, 1, 1)):
             a, c = bufs[src][oa:oa + n], outs[dst][oc:oc + n]
             plan.append((src, dst, a, c))
             want.append(expected_cast_launch(f"convert_vec<{DT_CODE[src]},{DT_CODE[dst]}>", ES[src], ES[dst], n,
@@ -301,28 +272,13 @@ def test_trace_shows_the_planned_kernels(tmp_path):
     for dt in V.DTYPES:
         plan.append((dt, dt, bufs[dt][:1000], outs[dt][:1000]))
         want.append((f"stream_vec<{DT_CODE[dt]},0,1,0,0>", -(-1000 * ES[dt] // 16 // 128), 128))
-    marker = torch.zeros(1, device="cuda")
-    torch.cuda.synchronize()
 
     def run_plan():
         for _, dst, a, c in plan:
             convert(a, dst, c)
         torch.cuda.synchronize()
 
-    # As in test_gpu_stream_dot.py: the plan runs twice, a fill kernel marks the start of the second pass, and the
-    # second pass is checked.
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        run_plan()
-        marker.fill_(1.0)
-        torch.cuda.synchronize()
-        run_plan()
-    trace = tmp_path / "trace.json"
-    prof.export_chrome_trace(str(trace))
-    events = sorted((e for e in json.loads(trace.read_text())["traceEvents"] if e.get("cat") in ("kernel", "gpu_memset")),
-                    key=lambda e: e["ts"])
-    m = max(i for i, e in enumerate(events) if "convert_vec" not in e["name"] and "stream_vec" not in e["name"])
-    assert events[m].get("cat") == "kernel" and "ill" in events[m]["name"], events[m]["name"]
-    got = [(_profiled_kernel_name(e["name"]), e["args"]["grid"][0], e["args"]["block"][0]) for e in events[m + 1:]]
+    got = kernels_after_marker(tmp_path, run_plan, ("convert_vec", "stream_vec"))
     assert len(got) == len(want), (len(got), len(want), got[:8])
     for g, w, p in zip(got, want, plan):
         assert g == w, (p[:2], g, w)

@@ -18,7 +18,6 @@ matches NaN as a class).  Outputs are poisoned beforehand and guard elements on 
 This module's name sorts after test_gpu_typecast.py: a module with profiler traces that runs before the parity and
 stream modules makes their traces lose kernels (DESIGN.md section 3).
 """
-import json
 import math
 
 import numpy as np
@@ -33,64 +32,24 @@ pytestmark = pytest.mark.gpu
 if has_gpu():
     import torch
 
+    from gpu_helpers import (DT_CODE, ES, F8_CODE, GUARD, LO, POISON, TORCH, M, _chains, _run, assert_guards,
+                             assert_matches, expected_cast_launch, hbm_n, kernels_after_marker, poisoned, tiled, to_dev)
+    from gpu_helpers import env  # noqa: F401  (the module-scoped fixture)
     from k8s_gpu_hpa_b200 import capi, vector_add as va
-    from test_gpu_parity import _profiled_kernel_name
-    from test_gpu_pdl_chains import LO, M, _chains, _run, env  # noqa: F401  (env: the module-scoped fixture)
-    from test_gpu_stream import GUARD, POISON, assert_guards, assert_matches, poisoned, tiled, to_dev
-    from test_gpu_typecast import expected_cast_launch
-
-    TORCH = {"f32": torch.float32, "f64": torch.float64, "f16": torch.float16, "bf16": torch.bfloat16}
-    TORCH8 = {"e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
 
 DTYPES = V.DTYPES
 FMTS = F.FORMATS8
-ES = V.SIZE
-DT_CODE = {"f32": 0, "f64": 1, "f16": 2, "bf16": 3}
-F8_CODE = {"e4m3": 0, "e5m2": 1}
 PAIRS = [("q", t, f) for t in DTYPES for f in FMTS] + [("d", t, f) for t in DTYPES for f in FMTS]
 PERIOD = 199_999
 
 
 # ------------------------------------------------------------------------------------------- helpers
-def to_dev8(bits, fmt):
-    return torch.from_numpy(np.ascontiguousarray(bits, np.uint8)).cuda().view(TORCH8[fmt])
-
-
-def tiled8(bits, n, fmt):
-    t = torch.from_numpy(np.ascontiguousarray(bits, np.uint8)).cuda()
-    t = t.repeat(-(-n // t.numel()))[:n] if n > t.numel() else t[:n].contiguous()
-    return t.view(TORCH8[fmt])
-
-
-def poisoned8(n, fmt, off=0):
-    buf = torch.empty(GUARD + off + n + GUARD, dtype=torch.uint8, device="cuda")
-    buf.fill_(POISON)
-    return buf, buf[GUARD + off:GUARD + off + n].view(TORCH8[fmt])
-
-
-def _nan8(u8, fmt):
-    m = u8 & 0x7F
-    return m == 0x7F if fmt == "e4m3" else m > 0x7C
-
-
-def assert_matches8(got, want, fmt, what="", chunk=1 << 30):
-    """FP8 bit patterns equal element by element on the device, NaN matching NaN as a class."""
-    assert got.numel() == want.numel()
-    for lo in range(0, got.numel(), chunk):
-        g, w = got[lo:lo + chunk].view(torch.uint8), want[lo:lo + chunk].view(torch.uint8)
-        bad = (g != w) & ~(_nan8(g, fmt) & _nan8(w, fmt))
-        if bool(bad.any()):
-            i = int(torch.nonzero(bad)[0])
-            raise AssertionError(f"{what}: {int(bad.sum())} mismatches, first at {lo + i} of {got.numel()}: "
-                                 f"got {int(g[i]):#04x} want {int(w[i]):#04x}")
-
-
 def random_fp8(n, rng):
     return rng.integers(0, 256, n, dtype=np.uint16).astype(np.uint8)
 
 
 def quantize(a, fmt, out, k=0, **kw):
-    return va.quantize_fp8(a, TORCH8[fmt], scale_exp=k, out=out, **kw)
+    return va.quantize_fp8(a, TORCH[fmt], scale_exp=k, out=out, **kw)
 
 
 def dequantize(a, dst, out, k=0, **kw):
@@ -99,10 +58,10 @@ def dequantize(a, dst, out, k=0, **kw):
 
 def check_quant(src, fmt, a_host, a_dev, k=0, off_c=0, what=""):
     n = a_host.size
-    buf, out = poisoned8(n, fmt, off_c)
+    buf, out = poisoned(n, fmt, off_c)
     quantize(a_dev, fmt, out, k)
     torch.cuda.synchronize()
-    assert_matches8(out, to_dev8(F.quantize(a_host, src, fmt, k), fmt), fmt, what)
+    assert_matches(out, to_dev(F.quantize(a_host, src, fmt, k), fmt), fmt, what)
     assert_guards(buf, GUARD + off_c, n, what)
 
 
@@ -113,11 +72,6 @@ def check_dequant(fmt, dst, bits, a_dev, k=0, off_c=0, what=""):
     torch.cuda.synchronize()
     assert_matches(out, to_dev(F.dequantize(bits, fmt, dst, k), dst), dst, what)
     assert_guards(buf, GUARD + off_c, n, what)
-
-
-def hbm_n(t):
-    """The smallest n in the HBM class of a pair with wide type t: the wide operand holds 2^25 four-byte words."""
-    return (1 << 25) * 4 // ES[t]
 
 
 def _amax_tensor(v=0.0):
@@ -148,17 +102,16 @@ def test_sizes_around_the_group_at_every_offset(kind, t, fmt):
             abuf, _ = poisoned(total, t)
             abuf[GUARD:GUARD + total].copy_(to_dev(host, t))
         else:
-            abuf, _ = poisoned8(total, fmt)
-            abuf[GUARD:GUARD + total].copy_(torch.from_numpy(host).cuda())
-            abuf = abuf.view(TORCH8[fmt])
+            abuf, _ = poisoned(total, fmt)
+            abuf[GUARD:GUARD + total].copy_(to_dev(host, fmt))
         for oc in offs_c:
             for n in sizes:
                 a, what = abuf[GUARD + oa:GUARD + oa + n], f"{kind} {t} {fmt} n={n} offsets A {oa} C {oc}"
                 if kind == "q":
-                    buf, out = poisoned8(n, fmt, oc)
+                    buf, out = poisoned(n, fmt, oc)
                     quantize(a, fmt, out, k)
                     torch.cuda.synchronize()
-                    assert_matches8(out, to_dev8(want_all[oa:oa + n], fmt), fmt, what)
+                    assert_matches(out, to_dev(want_all[oa:oa + n], fmt), fmt, what)
                 else:
                     buf, out = poisoned(n, t, oc)
                     dequantize(a, t, out, k)
@@ -182,7 +135,7 @@ def test_every_16_bit_pattern(src, fmt):
 @pytest.mark.parametrize("fmt", FMTS)
 def test_every_fp8_pattern(fmt, dst):
     bits = np.tile(np.arange(256, dtype=np.uint8), 5)      # several groups, so the vector body sees every pattern
-    a = to_dev8(bits, fmt)
+    a = to_dev(bits, fmt)
     for k in (-126, -1, 0, 1, 126):
         for off_c in (0, 1):
             check_dequant(fmt, dst, bits, a, k, off_c, f"{fmt}->{dst} all patterns, k={k}, C offset {off_c}")
@@ -217,23 +170,23 @@ def test_infinities_and_nans_from_every_source(src):
 @pytest.mark.parametrize("kind,t,fmt", PAIRS)
 def test_both_sides_of_the_hbm_edge(kind, t, fmt):
     """n = h - 1 and h at aligned pointers, then h + 37 with A and C one element past a 16-byte boundary."""
-    h = hbm_n(t)
+    h = hbm_n(ES[t])
     big = h + 37
     rng = np.random.default_rng([9, DT_CODE[t], F8_CODE[fmt], kind == "q"])
     k = -2 if kind == "q" else 2
     if kind == "q":
         block = V.random_bits(t, PERIOD, rng)
-        a, want = tiled(block, big + 1, t), tiled8(F.quantize(block, t, fmt, k), big + 1, fmt)
+        a, want = tiled(block, big + 1, t), tiled(F.quantize(block, t, fmt, k), big + 1, fmt)
     else:
         block = random_fp8(PERIOD, rng)
-        a, want = tiled8(block, big + 1, fmt), tiled(F.dequantize(block, fmt, t, k), big + 1, t)
+        a, want = tiled(block, big + 1, fmt), tiled(F.dequantize(block, fmt, t, k), big + 1, t)
     for n, off in ((h - 1, 0), (h, 0), (big, 1)):
         what = f"{kind} {t} {fmt} n={n} offset {off}"
         if kind == "q":
-            buf, out = poisoned8(n, fmt, off)
+            buf, out = poisoned(n, fmt, off)
             quantize(a[off:off + n], fmt, out, k)
             torch.cuda.synchronize()
-            assert_matches8(out, want[off:off + n], fmt, what)
+            assert_matches(out, want[off:off + n], fmt, what)
         else:
             buf, out = poisoned(n, t, off)
             dequantize(a[off:off + n], t, out, k)
@@ -258,8 +211,8 @@ def test_f16_e4m3_f16_beyond_32_bit_offsets():
     q.fill_(POISON)
     quantize(a, "e4m3", q.view(torch.float8_e4m3fn), 4)
     del a
-    want = tiled8(q_block, n, "e4m3")
-    assert_matches8(q.view(torch.float8_e4m3fn), want, "e4m3", "quantize, n = 2^32 + 4099")
+    want = tiled(q_block, n, "e4m3")
+    assert_matches(q.view(torch.float8_e4m3fn), want, "e4m3", "quantize, n = 2^32 + 4099")
     del want
     c = torch.empty(n, dtype=torch.float16, device="cuda")
     c.view(torch.uint8).fill_(POISON)
@@ -307,7 +260,7 @@ def test_amax(src):
     quantize(a, "e4m3", out, 0)
     torch.cuda.synchronize()
     assert float(m.item()) == -7.0
-    assert_matches8(out, to_dev8(F.quantize(finite, src, "e4m3", 0), "e4m3"), "e4m3", "amax NULL")
+    assert_matches(out, to_dev(F.quantize(finite, src, "e4m3", 0), "e4m3"), "e4m3", "amax NULL")
 
 
 # ------------------------------------------------------------------------------------------- arguments
@@ -373,10 +326,10 @@ def test_stream_op_quantize_dequantize_stream_op_on_one_stream():
             c = F.dequantize(F.quantize(b, src, fmt, k), fmt, dst, k)
             wants.append(X.stream("scale", dst, c, None, 0.5))
             amaxes.append(F.amax(b, src))
-        for n in ((1 << 20) + 5, hbm_n(src) + 5):
+        for n in ((1 << 20) + 5, hbm_n(ES[src]) + 5):
             a = tiled(a0, n, src)
             b = torch.empty_like(a)
-            q = torch.empty(n, dtype=TORCH8[fmt], device="cuda")
+            q = torch.empty(n, dtype=TORCH[fmt], device="cuda")
             c = torch.empty(n, dtype=TORCH[dst], device="cuda")
             ds = [torch.empty_like(c) for _ in scalars]
             ms = torch.zeros(len(scalars), dtype=torch.float64, device="cuda")
@@ -397,7 +350,7 @@ def test_captured_graph_replays_with_the_amax_reset_inside():
     cases = []
     for src, fmt, dst in (("f32", "e5m2", "f64"), ("f64", "e4m3", "f16"), ("bf16", "e4m3", "f32")):
         x = V.random_bits(src, 100_003, np.random.default_rng(DT_CODE[src] + 40))
-        bq, q = poisoned8(x.size, fmt, 1)
+        bq, q = poisoned(x.size, fmt, 1)
         bc, c = poisoned(x.size, dst, 3)
         cases.append((src, fmt, dst, x, to_dev(x, src), bq, q, bc, c, _amax_tensor(5.0)))
     g = torch.cuda.CUDAGraph()
@@ -413,7 +366,7 @@ def test_captured_graph_replays_with_the_amax_reset_inside():
     torch.cuda.synchronize()
     for r in range(2):
         for case in cases:
-            case[5].fill_(POISON)
+            case[5].view(torch.uint8).fill_(POISON)
             case[7].view(torch.uint8).fill_(POISON)
             case[9].fill_(1e300)
         g.replay()
@@ -421,7 +374,7 @@ def test_captured_graph_replays_with_the_amax_reset_inside():
         for src, fmt, dst, x, _, bq, q, bc, c, m in cases:
             what = f"{src}->{fmt}->{dst} replay {r}"
             qb = F.quantize(x, src, fmt, -4)
-            assert_matches8(q, to_dev8(qb, fmt), fmt, what)
+            assert_matches(q, to_dev(qb, fmt), fmt, what)
             assert_matches(c, to_dev(F.dequantize(qb, fmt, dst, -4), dst), dst, what)
             assert_guards(bq, GUARD + 1, x.size, what)
             assert_guards(bc, GUARD + 3, x.size, what)
@@ -459,14 +412,14 @@ def test_quantize_tail_reads_what_the_writer_wrote(env):
 def test_trace_shows_the_planned_kernels(tmp_path):
     """Per pair: n = 1000, the HBM class, n = 1001 in mixed phase and an odd n with a head.  Under the profiler the
     kernels after the marker are exactly the planned ones with their grid and block."""
-    nmax = max(hbm_n(t) for t in DTYPES) + 64
+    nmax = max(hbm_n(ES[t]) for t in DTYPES) + 64
     wide = {t: torch.zeros(nmax, dtype=TORCH[t], device="cuda") for t in DTYPES}
-    narrow = {f: torch.zeros(nmax, dtype=torch.uint8, device="cuda").view(TORCH8[f]) for f in FMTS}
-    narrow_out = {f: torch.zeros(nmax, dtype=torch.uint8, device="cuda").view(TORCH8[f]) for f in FMTS}
+    narrow = {f: torch.zeros(nmax, dtype=torch.uint8, device="cuda").view(TORCH[f]) for f in FMTS}
+    narrow_out = {f: torch.zeros(nmax, dtype=torch.uint8, device="cuda").view(TORCH[f]) for f in FMTS}
     wide_out = {t: torch.zeros(nmax, dtype=TORCH[t], device="cuda") for t in DTYPES}
     plan, want = [], []
     for kind, t, fmt in PAIRS:
-        for n, oa, oc in ((1000, 0, 0), (hbm_n(t), 0, 0), (1001, 0, 1), (4099, 1, 1)):
+        for n, oa, oc in ((1000, 0, 0), (hbm_n(ES[t]), 0, 0), (1001, 0, 1), (4099, 1, 1)):
             if kind == "q":
                 a, c = wide[t][oa:oa + n], narrow_out[fmt][oc:oc + n]
                 launch = (f"fp8_quant_vec<{DT_CODE[t]}>", ES[t], 1, n, a.data_ptr(), c.data_ptr())
@@ -475,9 +428,7 @@ def test_trace_shows_the_planned_kernels(tmp_path):
                 launch = (f"fp8_dequant_vec<{DT_CODE[t]}>", 1, ES[t], n, a.data_ptr(), c.data_ptr(), ES[t])
             plan.append((kind, t, fmt, a, c))
             want.append(expected_cast_launch(*launch))
-    marker = torch.zeros(1, device="cuda")
     amax = _amax_tensor()
-    torch.cuda.synchronize()
 
     def run_plan():
         for kind, t, fmt, a, c in plan:
@@ -487,18 +438,7 @@ def test_trace_shows_the_planned_kernels(tmp_path):
                 dequantize(a, t, c, 0)
         torch.cuda.synchronize()
 
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        run_plan()
-        marker.fill_(1.0)
-        torch.cuda.synchronize()
-        run_plan()
-    trace = tmp_path / "trace.json"
-    prof.export_chrome_trace(str(trace))
-    events = sorted((e for e in json.loads(trace.read_text())["traceEvents"] if e.get("cat") in ("kernel", "gpu_memset")),
-                    key=lambda e: e["ts"])
-    mk = max(i for i, e in enumerate(events) if "fp8_" not in e["name"])
-    assert events[mk].get("cat") == "kernel" and "ill" in events[mk]["name"], events[mk]["name"]
-    got = [(_profiled_kernel_name(e["name"]), e["args"]["grid"][0], e["args"]["block"][0]) for e in events[mk + 1:]]
+    got = kernels_after_marker(tmp_path, run_plan, ("fp8_",))
     assert len(got) == len(want), (len(got), len(want), got[:8])
     for g, w, p in zip(got, want, plan):
         assert g == w, (p[:3], g, w)

@@ -18,8 +18,6 @@ guard bytes on both sides of each must keep the poison.
 This module's name sorts after test_gpu_typecast_fp8.py: a module with profiler traces that runs before the parity
 and stream modules makes their traces lose kernels (DESIGN.md section 3).
 """
-import json
-
 import numpy as np
 import pytest
 
@@ -33,59 +31,38 @@ pytestmark = pytest.mark.gpu
 if has_gpu():
     import torch
 
+    from gpu_helpers import (DT_CODE, ES, F8_CODE, GUARD, LO, POISON, TORCH, M, _chains, _run, assert_guards,
+                             assert_matches, expected_mx_launch, hbm_n, kernels_after_marker, poisoned, tiled, to_dev)
+    from gpu_helpers import env  # noqa: F401  (the module-scoped fixture)
     from k8s_gpu_hpa_b200 import capi, vector_add as va
-    from test_gpu_parity import _profiled_kernel_name
-    from test_gpu_pdl_chains import LO, M, _chains, _run, env  # noqa: F401  (env: the module-scoped fixture)
-    from test_gpu_stream import GUARD, POISON, assert_guards, assert_matches, poisoned, tiled, to_dev
-    from test_gpu_typecast_fp8 import assert_matches8, poisoned8, tiled8, to_dev8
-
-    TORCH = {"f32": torch.float32, "f64": torch.float64, "f16": torch.float16, "bf16": torch.bfloat16}
-    TORCH8 = {"e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
 
 DTYPES = V.DTYPES
 FMTS = F.FORMATS8
-ES = V.SIZE
-DT_CODE = {"f32": 0, "f64": 1, "f16": 2, "bf16": 3}
-F8_CODE = {"e4m3": 0, "e5m2": 1}
 COMBOS = [(t, f, b, r) for t in DTYPES for f in FMTS for b in MX.BLOCKS for r in MX.RULES]
 PERIOD = 128 * 1563                       # a whole number of blocks, so a repeated period repeats its reference
 SCALE_BYTES = (0, 1, 126, 127, 128, 254, 255)
 
 
 # ------------------------------------------------------------------------------------------- helpers
-def poisoned_scales(count, off=0):
-    buf = torch.empty(GUARD + off + count + GUARD, dtype=torch.uint8, device="cuda")
-    buf.fill_(POISON)
-    return buf, buf[GUARD + off:GUARD + off + count]
-
-
 def quantize(a, fmt, block, rule, out, scales, **kw):
-    return va.quantize_mxfp8(a, TORCH8[fmt], block=block, scale_rule=rule, out=out, scales=scales, **kw)
+    return va.quantize_mxfp8(a, TORCH[fmt], block=block, scale_rule=rule, out=out, scales=scales, **kw)
 
 
 def dequantize(q, scales, dst, block, out, **kw):
     return va.dequantize_mxfp8(q, scales, TORCH[dst], block=block, out=out, **kw)
 
 
-def assert_scales(got, want, what):
-    assert got.numel() == want.numel(), what
-    bad = got != want
-    if bool(bad.any()):
-        i = int(torch.nonzero(bad)[0])
-        raise AssertionError(f"{what}: {int(bad.sum())} scale bytes differ, first at block {i}: got {int(got[i])} want {int(want[i])}")
-
-
 def check_quant(src, fmt, block, rule, a_host, a_dev, off_c=0, off_s=0, what=""):
     """Quantize a_dev into poisoned C and S at the given offsets; compare both with the reference of a_host.  Returns
     (q, s) as uint8 device tensors."""
     n = a_host.size
-    bq, q = poisoned8(n, fmt, off_c)
-    bs, s = poisoned_scales(MX.scale_count(n, block), off_s)
+    bq, q = poisoned(n, fmt, off_c)
+    bs, s = poisoned(MX.scale_count(n, block), "u8", off_s)
     quantize(a_dev, fmt, block, rule, q, s)
     torch.cuda.synchronize()
     wq, ws = MX.quantize(a_host, src, fmt, block, rule)
-    assert_matches8(q, to_dev8(wq, fmt), fmt, what)
-    assert_scales(s, torch.from_numpy(ws).cuda(), what)
+    assert_matches(q, to_dev(wq, fmt), fmt, what)
+    assert_matches(s, to_dev(ws, "u8"), "u8", what, nan_class=False)
     assert_guards(bq, GUARD + off_c, n, what)
     assert_guards(bs, GUARD + off_s, s.numel(), what + " (scales)")
     return q.view(torch.uint8), s
@@ -111,11 +88,6 @@ def random_scales(count, rng):
     return s
 
 
-def hbm_n(t):
-    """The smallest n in the HBM class of type t: 2^25 four-byte words."""
-    return (1 << 25) * 4 // ES[t]
-
-
 def at_offset(x_dev, off, torch_dtype):
     """A copy of x_dev `off` elements past a 16-byte boundary."""
     buf = torch.empty(x_dev.numel() + 16, dtype=torch_dtype, device="cuda")
@@ -139,7 +111,7 @@ def test_ragged_sizes_around_block_group_and_tile_edges(t, fmt, block, rule):
         check_quant(t, fmt, block, rule, host[:n], a[:n], 0, 0, f"quantize {t}->{fmt} block {block} {rule} n={n}")
         if rule == "ocp":
             nb = MX.scale_count(n, block)
-            check_dequant(fmt, t, block, bits[:n], sc[:nb], to_dev8(bits[:n], fmt), torch.from_numpy(sc[:nb]).cuda(), 0,
+            check_dequant(fmt, t, block, bits[:n], sc[:nb], to_dev(bits[:n], fmt), to_dev(sc[:nb], "u8"), 0,
                           f"dequantize {fmt}->{t} block {block} n={n}")
 
 
@@ -162,10 +134,10 @@ def test_every_offset_gives_the_bytes_of_offset_zero(t, fmt):
                 assert torch.equal(q, q0) and torch.equal(s, s0), f"{what} offsets A {oa} C {oc}: not the bytes of offset 0"
         bits, sc = random_fp8(n, rng), random_scales(MX.scale_count(n, block), rng)
         want = to_dev(MX.dequantize(bits, sc, fmt, t, block), t)
-        q0 = to_dev8(bits, fmt)
+        q0 = to_dev(bits, fmt)
         for oa in range(16):
-            q = at_offset(q0, oa, TORCH8[fmt])
-            s = at_offset(torch.from_numpy(sc).cuda(), 1 + oa % 3, torch.uint8)
+            q = at_offset(q0, oa, TORCH[fmt])
+            s = at_offset(to_dev(sc, "u8"), 1 + oa % 3, torch.uint8)
             for oc in range(16 // ES[t]):
                 what = f"dequantize {fmt}->{t} block {block} n={n} offsets A {oa} C {oc}"
                 buf, out = poisoned(n, t, oc)
@@ -187,7 +159,7 @@ def test_named_sets(t, fmt, block, rule):
     assert torch.equal(q, q1) and torch.equal(s, s1)
     # back into the source type: the FP8 values scaled back, rounded once
     qh, sh = q.cpu().numpy(), s.cpu().numpy()
-    check_dequant(fmt, t, block, qh, sh, q.view(TORCH8[fmt]), s, 0, f"{fmt}->{t} block {block} named sets back")
+    check_dequant(fmt, t, block, qh, sh, q.view(TORCH[fmt]), s, 0, f"{fmt}->{t} block {block} named sets back")
 
 
 @pytest.mark.parametrize("fmt", FMTS)
@@ -209,14 +181,14 @@ def test_every_16_bit_pattern(src, fmt):
 def test_every_fp8_pattern_under_the_extreme_scale_bytes(fmt, dst):
     """7168 elements: every pattern meets every one of the scale bytes (256 / block and 7 are coprime)."""
     bits = np.tile(np.arange(256, dtype=np.uint8), 28)
-    q = to_dev8(bits, fmt)
+    q = to_dev(bits, fmt)
     for block in MX.BLOCKS:
         sc = np.resize(np.array(SCALE_BYTES, np.uint8), bits.size // block)
-        s = torch.from_numpy(sc).cuda()
+        s = to_dev(sc, "u8")
         for off_c in (0, 1):
             check_dequant(fmt, dst, block, bits, sc, q, s, off_c, f"{fmt}->{dst} all patterns, block {block}, C offset {off_c}")
     sc = np.full(bits.size // 32, 0xFF, np.uint8)
-    out = dequantize(q, torch.from_numpy(sc).cuda(), dst, 32, None)
+    out = dequantize(q, to_dev(sc, "u8"), dst, 32, None)
     assert bool(torch.isnan(out).all())
 
 
@@ -230,7 +202,7 @@ def test_round_trip_and_unrelated_blocks(fmt):
         a = np.ldexp(F.DECODE[fmt][rng.choice(finite, nb * block)], np.repeat(rng.integers(-90, 90, nb), block))
         for src in ("f64", "f32"):
             host = a.astype(X.STORAGE[src])
-            q, s = va.quantize_mxfp8(to_dev(host, src), TORCH8[fmt], block=block, scale_rule="nosat")
+            q, s = va.quantize_mxfp8(to_dev(host, src), TORCH[fmt], block=block, scale_rule="nosat")
             back = va.dequantize_mxfp8(q, s, TORCH[src], block=block)
             torch.cuda.synchronize()
             assert_matches(back, to_dev(host, src), src, f"round trip {src} {fmt} block {block}", nan_class=False)
@@ -252,16 +224,16 @@ def _periodic_quant_want(host, t, fmt, block, rule, off, n):
     repeated, with the short last block computed from the elements it really holds."""
     rolled = np.roll(host, -off)
     wq, ws = MX.quantize(rolled, t, fmt, block, rule)
-    q = tiled8(wq, n, fmt).view(torch.uint8).clone()
-    s = torch.from_numpy(ws).cuda()
+    q = tiled(wq, n, fmt).view(torch.uint8).clone()
+    s = to_dev(ws, "u8")
     nb = MX.scale_count(n, block)
     s = s.repeat(-(-nb // s.numel()))[:nb].clone()
     tail = n - n % block
     if tail < n:
         tq, ts = MX.quantize(rolled[np.arange(tail, n) % host.size], t, fmt, block, rule)
-        q[tail:] = torch.from_numpy(tq).cuda()
+        q[tail:] = to_dev(tq, "u8")
         s[-1] = int(ts[0])
-    return q.view(TORCH8[fmt]), s
+    return q.view(TORCH[fmt]), s
 
 
 @pytest.mark.parametrize("fmt", FMTS)
@@ -270,7 +242,7 @@ def _periodic_quant_want(host, t, fmt, block, rule, off, n):
 def test_both_sides_of_the_hbm_edge(kind, t, fmt):
     """n = h - 1 and h at aligned pointers (h - 1 ends in a short block), then h + 37 with A and C one element past a
     16-byte boundary (the edge path at full size)."""
-    h = hbm_n(t)
+    h = hbm_n(ES[t])
     big = h + 37
     block, rule = (32, "ocp") if fmt == "e4m3" else (128, "nosat")
     rng = np.random.default_rng([9, DT_CODE[t], F8_CODE[fmt], kind == "q"])
@@ -279,18 +251,18 @@ def test_both_sides_of_the_hbm_edge(kind, t, fmt):
         a = tiled(host, big + 1, t)
     else:
         host, sc = random_fp8(PERIOD, rng), random_scales(PERIOD // block, rng)
-        a = tiled8(host, big + 1, fmt)
+        a = tiled(host, big + 1, fmt)
     for n, off in ((h - 1, 0), (h, 0), (big, 1)):
         what = f"{kind} {t} {fmt} block {block} n={n} offset {off}"
         nb = MX.scale_count(n, block)
         if kind == "q":
-            bq, q = poisoned8(n, fmt, off)
-            bs, s = poisoned_scales(nb, off)
+            bq, q = poisoned(n, fmt, off)
+            bs, s = poisoned(nb, "u8", off)
             quantize(a[off:off + n], fmt, block, rule, q, s)
             torch.cuda.synchronize()
             wq, ws = _periodic_quant_want(host, t, fmt, block, rule, off, n)
-            assert_matches8(q, wq, fmt, what)
-            assert_scales(s, ws, what)
+            assert_matches(q, wq, fmt, what)
+            assert_matches(s, ws, "u8", what, nan_class=False)
             assert_guards(bq, GUARD + off, n, what)
             assert_guards(bs, GUARD + off, nb, what + " (scales)")
             del bq, q, wq
@@ -298,7 +270,7 @@ def test_both_sides_of_the_hbm_edge(kind, t, fmt):
             # the view starts at element `off` of the period; its blocks start there too, with the period's scales
             rolled = np.roll(host, -off)
             want = tiled(MX.dequantize(rolled, sc, fmt, t, block), n, t)
-            s = torch.from_numpy(sc).cuda()
+            s = to_dev(sc, "u8")
             s = s.repeat(-(-nb // s.numel()))[:nb].contiguous()
             buf, out = poisoned(n, t, off)
             dequantize(a[off:off + n], s, t, block, out)
@@ -320,12 +292,12 @@ def test_f16_e4m3_f16_beyond_32_bit_offsets():
     a = tiled(host, n, "f16")
     q = torch.empty(n, dtype=torch.uint8, device="cuda")
     q.fill_(POISON)
-    bs, s = poisoned_scales(MX.scale_count(n, 32))
+    bs, s = poisoned(MX.scale_count(n, 32), "u8")
     quantize(a, "e4m3", 32, "ocp", q.view(torch.float8_e4m3fn), s)
     del a
     wq, ws = _periodic_quant_want(host, "f16", "e4m3", 32, "ocp", 0, n)
-    assert_matches8(q.view(torch.float8_e4m3fn), wq, "e4m3", "quantize, n = 2^32 + 4099")
-    assert_scales(s, ws, "quantize, n = 2^32 + 4099")
+    assert_matches(q.view(torch.float8_e4m3fn), wq, "e4m3", "quantize, n = 2^32 + 4099")
+    assert_matches(s, ws, "u8", "quantize, n = 2^32 + 4099", nan_class=False)
     assert_guards(bs, GUARD, s.numel(), "scales")
     del wq
     c = torch.empty(n, dtype=torch.float16, device="cuda")
@@ -408,10 +380,10 @@ def test_stream_op_quantize_dequantize_stream_op_on_one_stream():
         for s in scalars:
             qh, sh = MX.quantize(X.stream("scale", src, a0, None, s), src, fmt, block, rule)
             wants.append(X.stream("scale", dst, MX.dequantize(qh, sh, fmt, dst, block), None, 0.5))
-        for n in (21 * period, -(-(hbm_n(src) + 5) // period) * period):
+        for n in (21 * period, -(-(hbm_n(ES[src]) + 5) // period) * period):
             a = tiled(a0, n, src)
             b = torch.empty_like(a)
-            q = torch.empty(n, dtype=TORCH8[fmt], device="cuda")
+            q = torch.empty(n, dtype=TORCH[fmt], device="cuda")
             sc = torch.empty(n // block, dtype=torch.uint8, device="cuda")
             c = torch.empty(n, dtype=TORCH[dst], device="cuda")
             ds = [torch.empty_like(c) for _ in scalars]
@@ -432,8 +404,8 @@ def test_captured_graph_replays():
     for src, fmt, dst, block, rule in (("f32", "e5m2", "f64", 32, "nosat"), ("f64", "e4m3", "f16", 64, "ocp"),
                                        ("bf16", "e4m3", "f32", 128, "ocp")):
         x = V.random_bits(src, 100_003, np.random.default_rng(DT_CODE[src] + 40))
-        bq, q = poisoned8(x.size, fmt, 16)
-        bs, s = poisoned_scales(MX.scale_count(x.size, block), 1)
+        bq, q = poisoned(x.size, fmt, 16)
+        bs, s = poisoned(MX.scale_count(x.size, block), "u8", 1)
         bc, c = poisoned(x.size, dst, 16 // ES[dst])
         cases.append((src, fmt, dst, block, rule, x, to_dev(x, src), bq, q, bs, s, bc, c))
     g = torch.cuda.CUDAGraph()
@@ -448,7 +420,7 @@ def test_captured_graph_replays():
     torch.cuda.synchronize()
     for r in range(2):
         for case in cases:
-            case[7].fill_(POISON)
+            case[7].view(torch.uint8).fill_(POISON)
             case[9].fill_(POISON)
             case[11].view(torch.uint8).fill_(POISON)
         g.replay()
@@ -456,8 +428,8 @@ def test_captured_graph_replays():
         for src, fmt, dst, block, rule, x, _, bq, q, bs, s, bc, c in cases:
             what = f"{src}->{fmt}->{dst} block {block} replay {r}"
             wq, ws = MX.quantize(x, src, fmt, block, rule)
-            assert_matches8(q, to_dev8(wq, fmt), fmt, what)
-            assert_scales(s, torch.from_numpy(ws).cuda(), what)
+            assert_matches(q, to_dev(wq, fmt), fmt, what)
+            assert_matches(s, to_dev(ws, "u8"), "u8", what, nan_class=False)
             assert_matches(c, to_dev(MX.dequantize(wq, ws, fmt, dst, block), dst), dst, what)
             assert_guards(bq, GUARD + 16, x.size, what)
             assert_guards(bs, GUARD + 1, s.numel(), what)
@@ -485,24 +457,10 @@ def test_quantize_tail_reads_what_the_writer_wrote(env):
 
 
 # ------------------------------------------------------------------------------------------- trace
-def expected_mx_launch(kind, es, n, block, aligned):
-    """(kernel, grid, block) of launch_mx_typed (b200va_typed.cu)."""
-    nblocks = -(-n // block)
-    if kind == "q":
-        ngroups = n // block * (block // 16) if aligned else 0
-        units, edges = ngroups, nblocks - ngroups * 16 // block
-    else:
-        ngroups = n // 16 if aligned else 0
-        units, edges = ngroups * es, n - ngroups * 16
-    threads, unroll = (512, 2) if n >= (1 << 25) * 4 // es else (256, 1)
-    blocks = max(-(-units // (threads * unroll)), -(-edges // threads))
-    return f"mx_{'quant' if kind == 'q' else 'dequant'}_vec<{es}>", max(1, min(blocks, 2 ** 31 - 1)), threads
-
-
 def test_trace_shows_the_planned_kernels(tmp_path):
     """Per type, direction and block: n = 1000 and the HBM class on the vector body, n = 4099 on the edge path.  Under
     the profiler the kernels after the marker are exactly the planned ones with their grid and block."""
-    nmax = max(hbm_n(t) for t in DTYPES) + 64
+    nmax = max(hbm_n(ES[t]) for t in DTYPES) + 64
     wide = {t: torch.zeros(nmax, dtype=TORCH[t], device="cuda") for t in DTYPES}
     narrow = torch.zeros(nmax, dtype=torch.uint8, device="cuda")
     scales = torch.full((nmax // 32 + 2,), 127, dtype=torch.uint8, device="cuda")
@@ -510,13 +468,11 @@ def test_trace_shows_the_planned_kernels(tmp_path):
     for kind in ("q", "d"):
         for t in DTYPES:
             for block in MX.BLOCKS:
-                for n, off in ((1000, 0), (hbm_n(t), 0), (4099, 1)):
+                for n, off in ((1000, 0), (hbm_n(ES[t]), 0), (4099, 1)):
                     fmt = FMTS[(n + block) % 2]
-                    w, f8 = wide[t][off:off + n], narrow[off:off + n].view(TORCH8[fmt])
+                    w, f8 = wide[t][off:off + n], narrow[off:off + n].view(TORCH[fmt])
                     plan.append((kind, t, fmt, block, w, f8, scales[1:1 + MX.scale_count(n, block)]))
                     want.append(expected_mx_launch(kind, ES[t], n, block, off == 0))
-    marker = torch.zeros(1, device="cuda")
-    torch.cuda.synchronize()
 
     def run_plan():
         for kind, t, fmt, block, w, f8, s in plan:
@@ -526,20 +482,7 @@ def test_trace_shows_the_planned_kernels(tmp_path):
                 dequantize(f8, s, t, block, w)
         torch.cuda.synchronize()
 
-    # As in test_gpu_typecast_fp8.py: the plan runs twice, a fill kernel marks the start of the second pass, and the
-    # second pass is checked.
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        run_plan()
-        marker.fill_(1.0)
-        torch.cuda.synchronize()
-        run_plan()
-    trace = tmp_path / "trace.json"
-    prof.export_chrome_trace(str(trace))
-    events = sorted((e for e in json.loads(trace.read_text())["traceEvents"] if e.get("cat") in ("kernel", "gpu_memset")),
-                    key=lambda e: e["ts"])
-    mk = max(i for i, e in enumerate(events) if "mx_" not in e["name"])
-    assert events[mk].get("cat") == "kernel" and "ill" in events[mk]["name"], events[mk]["name"]
-    got = [(_profiled_kernel_name(e["name"]), e["args"]["grid"][0], e["args"]["block"][0]) for e in events[mk + 1:]]
+    got = kernels_after_marker(tmp_path, run_plan, ("mx_",))
     assert len(got) == len(want), (len(got), len(want), got[:8])
     for g, w, p in zip(got, want, plan):
         assert g == w, (p[:4], g, w)

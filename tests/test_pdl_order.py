@@ -12,10 +12,10 @@ the first ACQBULK of each kernel:
 The kernels without ACQBULK are exactly the ones the library launches without the PDL attribute.
 """
 import re
-import subprocess
 
 import pytest
 
+import sass
 from k8s_gpu_hpa_b200 import capi
 
 # launched with <<<>>> (no PDL attribute): the K0 control, the mixed-phase stream op, the support kernels
@@ -26,33 +26,16 @@ GLOBAL_READ = re.compile(r"(LDG|LD\.E|LD\b|UBLKCP\.S\.G|UTMALDG)")
 # every other instruction that names memory must be one of these before the wait
 ALLOWED = re.compile(r"(LDC|ULDC|PREEXIT|UBLKPF\.L2|CREATEPOLICY)\b")
 MEMORY = re.compile(r"(LD|ST|ATOM|RED|UBLK|UTMA|SYNCS|SU|TLD|TEX|CCTL|PREEXIT|MEMBAR|FENCE)")
-OPCODE = re.compile(r"/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)")
-
-
-def _parse(mangled: str) -> tuple[str, list[int]]:
-    """_ZN6b200va8vadd_vecILi4ELi1ELi0ELi1ELi1EEEv... -> ("vadd_vec", [4, 1, 0, 1, 1])."""
-    m = re.match(r"_ZN6b200va(\d+)", mangled)
-    assert m, mangled
-    name = mangled[m.end():m.end() + int(m.group(1))]
-    targs = re.match(r"I((?:L[a-z]\d+E)+)E", mangled[m.end() + len(name):])
-    return name, [int(v) for v in re.findall(r"L[a-z](\d+)E", targs.group(1))] if targs else []
-
-
-def _kernels(path: str) -> dict[str, list[str]]:
-    """Mangled name -> the kernel's opcodes in text order."""
-    sass = subprocess.run(["cuobjdump", "-sass", path], capture_output=True, text=True, check=True).stdout
-    parts = re.split(r"^\s*Function : (\S+)\s*$", sass, flags=re.M)
-    out = {}
-    for fn, body in zip(parts[1::2], parts[2::2]):
-        assert fn not in out, fn
-        out[fn] = OPCODE.findall(body)
-        assert out[fn], fn
-    return out
 
 
 @pytest.fixture(scope="module", params=["production", "tune"])
 def kernels(request):
-    return _kernels(capi.LIB_PATH if request.param == "production" else capi.TUNE_LIB_PATH)
+    """Mangled name -> the kernel's opcodes in text order."""
+    path = capi.LIB_PATH if request.param == "production" else capi.TUNE_LIB_PATH
+    out = {fn: sass.opcodes(body) for fn, body in sass.functions(path).items()}
+    for fn, ops in out.items():
+        assert ops, fn
+    return out
 
 
 def _early_loads(name: str, targs: list[int]) -> bool:
@@ -60,13 +43,13 @@ def _early_loads(name: str, targs: list[int]) -> bool:
 
 
 def test_kernels_without_a_wait_are_the_ones_launched_without_pdl(kernels):
-    names = {_parse(fn)[0] for fn in kernels}
+    names = {sass.parse(fn)[0] for fn in kernels}
     assert {"vadd_vec", "vadd_vec_dyn", "vadd_tma", "vadd_tma_dyn", "vadd_scalar_unrolled", "stream_vec", "convert_vec",
             "dot_vec", "dot_scalar", "dot_final", "probe_read2", "probe_fill", "probe_copy"} <= names
-    no_wait = {_parse(fn)[0] for fn, ops in kernels.items() if "ACQBULK" not in ops}
+    no_wait = {sass.parse(fn)[0] for fn, ops in kernels.items() if "ACQBULK" not in ops}
     assert no_wait == NO_WAIT
     for fn, ops in kernels.items():
-        if _parse(fn)[0] in NO_WAIT:
+        if sass.parse(fn)[0] in NO_WAIT:
             assert "ACQBULK" not in ops and "PREEXIT" not in ops, fn
 
 
@@ -78,7 +61,7 @@ def test_nothing_writes_global_memory_before_the_wait(kernels):
     for fn, ops in kernels.items():
         if "ACQBULK" not in ops:
             continue
-        name, targs = _parse(fn)
+        name, targs = sass.parse(fn)
         before = ops[:ops.index("ACQBULK")]
         writes = [o for o in before if GLOBAL_WRITE.match(o)]
         if name == "vadd_vec_dyn" and targs[4] == 1:
@@ -95,7 +78,7 @@ def test_only_the_early_load_forms_load_before_the_wait(kernels):
     for fn, ops in kernels.items():
         if "ACQBULK" not in ops:
             continue
-        name, targs = _parse(fn)
+        name, targs = sass.parse(fn)
         before = ops[:ops.index("ACQBULK")]
         loads = [o for o in before if GLOBAL_READ.match(o)]
         if _early_loads(name, targs):

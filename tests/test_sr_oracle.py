@@ -17,7 +17,6 @@ stochastic-rounding kernel's SASS.
 """
 import math
 import re
-import subprocess
 from fractions import Fraction
 
 import numpy as np
@@ -31,6 +30,7 @@ from oracle import sr_exact as S
 from oracle import stream_exact as X
 
 import k8s_gpu_hpa_b200 as pkg  # noqa: F401  (the session fixture has built the library)
+import sass
 from k8s_gpu_hpa_b200 import capi
 
 TWO32 = 1 << 32
@@ -381,9 +381,7 @@ def test_entry_points_fail_without_a_gpu_and_write_nothing():
 
 
 def _sr_functions(path: str) -> dict[str, str]:
-    sass = subprocess.run(["cuobjdump", "-sass", path], capture_output=True, text=True, check=True).stdout
-    parts = re.split(r"^\s*Function : (\S+)\s*$", sass, flags=re.M)
-    return {fn: body for fn, body in zip(parts[1::2], parts[2::2]) if "sr_cast_vec" in fn}
+    return {fn: body for fn, body in sass.functions(path).items() if "sr_cast_vec" in fn}
 
 
 @pytest.mark.parametrize("path", ["production", "tune"])
