@@ -110,9 +110,12 @@ namespace {
 
 // ----------------------------------------------------------------------- kernel pick
 // What each library carries.  libb200va.so carries the production set: what AUTO and the named variants
-// resolve to, plus close neighbours the parity tests run.  -DB200VA_TUNE_MATRIX (libb200va_tune.so, the A/B
-// tool's library) carries every combination of b200va_tune_t.  The pick below instantiates exactly the
-// kernels these predicates admit; any other combination gives nullptr, and so B200VA_ERR_VARIANT.
+// resolve to, plus their close neighbours in load hint, store hint, unroll and early loads, which
+// b200va_add_f32_tuned reaches.  -DB200VA_TUNE_MATRIX (libb200va_tune.so, the A/B tool's library) carries every
+// combination of b200va_tune_t.  The pick below instantiates exactly the kernels these predicates admit; any
+// other combination gives nullptr, and so B200VA_ERR_VARIANT.  tests/test_kernel_inventory.py restates the
+// predicates and checks them against each library's SASS; tests/test_gpu_tune_matrix.py runs every kernel of
+// both libraries against the oracle.
 template <int VW, int UNROLL, int LD, int ST, int EARLY, int SCHED>
 constexpr bool carries_vec()
 {

@@ -110,6 +110,60 @@ def geometry(t, n, lib=None):
     return rc, grid.value, block.value
 
 
+def expected_add_launch(t, n, pa, pb, pc, lib=None):
+    """(return code, kernel, grid, block) of plan_launch (b200va_add.cu) for tune t, every field of its kind set, adding
+    n elements at addresses pa and pb into pc.  The alias rules (.nc loads become plain, early register loads the L2
+    prefetch, when C is A or B), the vector width and head (K3 drops to the 16-byte body, mixed phase to K4 at
+    256 x 8) are restated here.  The grid is b200va_geometry's for the vector body alone, n_eff = nvec * vw elements
+    with the effective tune: its notional aligned operands have no head, so they give the same tiles."""
+    e = capi.Tune(**t.as_dict())
+    if pc in (pa, pb):
+        if e.ld_hint == 4:
+            e.ld_hint = 0
+        if e.early_loads == 1:
+            e.early_loads = 2
+    vw = {capi.K3_VEC256: 8, capi.K1_VEC128: 4, capi.K2_TMA: 4}.get(e.kind, 0)
+    head = 0
+    while vw:
+        mask = vw * 4 - 1
+        if pa & mask == pb & mask == pc & mask:
+            head = ((vw * 4 - (pa & mask)) & mask) // 4
+            break
+        vw = 4 if vw == 8 else 0
+    n_eff = n
+    if vw:
+        n_eff = (n - min(head, n)) // vw * vw
+        if e.kind == capi.K3_VEC256 and vw == 4:
+            e.kind = capi.K1_VEC128
+    elif e.kind not in (capi.K0_SCALAR, capi.K4_SCALAR_MLP):
+        e.kind, e.threads, e.unroll = capi.K4_SCALAR_MLP, 256, 8
+    rc, grid, block = geometry(e, n_eff, lib)
+    return rc, e.kernel_name(), grid, block
+
+
+def expected_stream_launch(op, dtype, n, head=0, override=None):
+    """(kernel, grid, block) launch_stream_typed (b200va_typed.cu) picks for n elements whose vector body starts head
+    elements in.  override: (threads, unroll, skip_l1_stores) of B200VA_STREAM_GEOMETRY, which only the tune library
+    reads; one it does not accept leaves the table's plan."""
+    m = n * ES[dtype] // 4
+    binary = op in ("add", "triad")
+    if m >= 1 << 25:
+        threads, unroll, st = (512, 1, 1) if binary else (1024, 2, 1)
+    elif m > 1 << 23:
+        threads, unroll, st = 128, 2, 0
+    elif m >= 1 << 21:
+        threads, unroll, st = 256, 2, 0
+    elif m >= 1 << 19:
+        threads, unroll, st = 512, 1, 0
+    else:
+        threads, unroll, st = 128, 1, 0
+    if override and 32 <= override[0] <= 1024 and override[0] % 32 == 0 and override[1] in (1, 2, 4):
+        threads, unroll, st = override[0], override[1], int(override[2] != 0)
+    nvec = (n - min(head, n)) * ES[dtype] // 16
+    grid = max(1, -(-nvec // (threads * unroll)))
+    return f"stream_vec<{DT_CODE[dtype]},{capi.OPS[op]},{unroll},0,{st}>", grid, threads
+
+
 def k1d_tunes():
     """The K1d (dynamic tile scheduler) tunes the production library carries."""
     return (capi.Tune(kind=capi.K1_VEC128, threads=256, unroll=2, st_hint=1, scheduler=1),

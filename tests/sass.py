@@ -9,6 +9,8 @@ import re
 import subprocess
 
 OPCODE = re.compile(r"/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)")
+# one instruction line: its address, the instruction text, its encoding word
+INSTRUCTION = re.compile(r"^\s*/\*[0-9a-f]{4,}\*/\s+(.*?)\s*;?\s*/\*\s*0x[0-9a-f]{16}\s*\*/\s*$", re.M)
 
 
 @functools.lru_cache(maxsize=None)
@@ -33,6 +35,11 @@ def opcodes(body: str) -> list[str]:
     return OPCODE.findall(body)
 
 
+def instructions(body: str) -> list[str]:
+    """The instruction text of a function's SASS in text order, without addresses and encodings."""
+    return INSTRUCTION.findall(body)
+
+
 def parse(mangled: str) -> tuple[str, list[int]]:
     """_ZN6b200va8vadd_vecILi4ELi1ELi0ELi1ELi1EEEv... -> ("vadd_vec", [4, 1, 0, 1, 1])."""
     m = re.match(r"_ZN6b200va(\d+)", mangled)
@@ -40,6 +47,13 @@ def parse(mangled: str) -> tuple[str, list[int]]:
     name = mangled[m.end():m.end() + int(m.group(1))]
     targs = re.match(r"I((?:L[a-z]\d+E)+)E", mangled[m.end() + len(name):])
     return name, [int(v) for v in re.findall(r"L[a-z](\d+)E", targs.group(1))] if targs else []
+
+
+def kernel_name(mangled: str) -> str:
+    """A kernel's name as a profiler trace gives it, in Tune.kernel_name()'s form: "vadd_vec<4,1,0,1,1>",
+    "vadd_tma_dyn<1,0>" (bools as 0/1), "vadd_scalar"."""
+    name, targs = parse(mangled)
+    return f"{name}<{','.join(map(str, targs))}>" if targs else name
 
 
 def ptx(path: str) -> str:

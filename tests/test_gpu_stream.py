@@ -26,8 +26,8 @@ if has_gpu():
     import torch
 
     import k8s_gpu_hpa_b200 as pkg
-    from gpu_helpers import (DT_CODE, ES, GUARD, POISON, TORCH, assert_guards, assert_matches, kernels_after_marker,
-                             poisoned, tiled, to_dev)
+    from gpu_helpers import (DT_CODE, ES, GUARD, POISON, TORCH, assert_guards, assert_matches, expected_stream_launch,
+                             kernels_after_marker, poisoned, tiled, to_dev)
     from k8s_gpu_hpa_b200 import capi, vector_add as va
 
 OPS = ["copy", "scale", "add", "triad"]
@@ -73,24 +73,6 @@ def class_edges(dtype):
         n = n_from(dtype, m)
         out += [n - 1, n]
     return out
-
-
-def expected_launch(op, dtype, n):
-    """(kernel, grid, block) launch_stream_typed picks for n elements on 16-byte-aligned pointers."""
-    m = n * ES[dtype] // 4
-    if m >= 1 << 25:
-        threads, unroll, st = (512, 1, 1) if op in BINARY else (1024, 2, 1)
-    elif m > 1 << 23:
-        threads, unroll, st = 128, 2, 0
-    elif m >= 1 << 21:
-        threads, unroll, st = 256, 2, 0
-    elif m >= 1 << 19:
-        threads, unroll, st = 512, 1, 0
-    else:
-        threads, unroll, st = 128, 1, 0
-    nvec = n * ES[dtype] // 16
-    grid = max(1, -(-nvec // (threads * unroll)))
-    return f"stream_vec<{DT_CODE[dtype]},{OP_CODE[op]},{unroll},0,{st}>", grid, threads
 
 
 def period_inputs(op, dtype, seed, period=PERIOD):
@@ -218,7 +200,7 @@ def test_every_stream_kernel_of_the_library_is_launched_with_the_dispatchers_geo
         for op in OPS:
             for n in sizes:
                 plan.append((op, dtype, n, 0))
-                want.append(expected_launch(op, dtype, n))
+                want.append(expected_stream_launch(op, dtype, n))
             plan.append((op, dtype, 1001, 1))                 # A one element past C: the scalar fallback
             want.append((f"stream_scalar<{DT_CODE[dtype]},{OP_CODE[op]}>", -(-1001 // 256), 256))
     bufs = {}
@@ -450,7 +432,7 @@ def test_small_launch_reading_the_end_of_a_large_one(dtype):
     scalars = [1.0 + k / 8 for k in range(10)]
     for s, (_, d) in zip(scalars, outs):
         run("scale", a, None, c, s, stream=st)
-        run("add", c[n - m:], b, d, stream=st)      # expected_launch: a stream_vec kernel, launched with PDL
+        run("add", c[n - m:], b, d, stream=st)      # expected_stream_launch: a stream_vec kernel, launched with PDL
     st.synchronize()
     for k, (s, (obuf, d)) in enumerate(zip(scalars, outs)):
         want = X.stream("add", dtype, X.stream("scale", dtype, tail, None, s), pb)
