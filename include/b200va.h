@@ -50,7 +50,7 @@ extern "C" {
 #define B200VA_ERR_VARIANT     (-4)   /* unknown kernel variant / unsupported tune combo  */
 #define B200VA_ERR_NO_DEVICE   (-5)   /* no CUDA device / not an sm_90 device             */
 #define B200VA_ERR_VERIFY      (-6)   /* result verification failed (a6)                  */
-#define B200VA_ERR_NOMEM       (-7)   /* host allocation failed                           */
+#define B200VA_ERR_NOMEM       (-7)   /* host allocation failed; captured-counter pool empty */
 #define B200VA_ERR_CUDA_BASE   (-1000) /* code = -(1000 + cudaError_t)                    */
 /* Which combinations a library carries: libb200va.so ships the production set (what
  * B200VA_K_AUTO and the named variants resolve to, plus a few neighbours); the full
@@ -127,7 +127,16 @@ int         b200va_geometry(const b200va_tune_t *tune, size_t n, int device,
 /* ---- a4 + a5: the vectorAdd kernel and its launch geometry -------------------------
  * Replaces `vectorAdd<<<blocksPerGrid, threadsPerBlock>>>(d_A, d_B, d_C, numElements)`
  * of the image's binary (invoked at cuda-test-deployment.yaml:19).
- * dA, dB, dC: device pointers, 4-byte aligned; any n >= 0; dC may equal dA or dB. */
+ * dA, dB, dC: device pointers, 4-byte aligned; any n >= 0; dC may equal dA or dB.
+ * Capture.  b200va_add_f32, b200va_add_f32_ex and b200va_add_f32_tuned are capturable in a CUDA graph, also as
+ * the first call of a process and under every capture mode: the one-time setup of the dynamic tile scheduler's
+ * counters runs in relaxed capture mode on a private stream.  A dynamically scheduled launch (variant K2,
+ * scheduler = 1) captured into a graph takes a ticket counter that the graph holds until it and every executable
+ * instance of it are destroyed; no direct launch is handed it meanwhile.  So the executable instances of one
+ * captured graph must not run at the same time, and each device lends at most 16384 such counters at once: one
+ * more is refused with B200VA_ERR_NOMEM.  b200va_add_f32_loop with graph_batch > 1 and b200va_loop_create
+ * allocate and synchronize, and are not capturable: the former returns -(1000 + cudaErrorStreamCaptureUnsupported)
+ * when `stream` is capturing. */
 int b200va_add_f32(const float *dA, const float *dB, float *dC, size_t n,
                    int variant, void *stream);
 int b200va_add_f32_tuned(const float *dA, const float *dB, float *dC, size_t n,

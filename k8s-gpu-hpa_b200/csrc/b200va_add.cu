@@ -3,6 +3,7 @@
 // probes.  The only unit that includes b200va_kernels.cuh.
 #include <map>
 #include <utility>
+#include <vector>
 
 #include "b200va_internal.h"
 #include "b200va_kernels.cuh"
@@ -311,35 +312,127 @@ int plan_grid(const b200va_tune_t& t, const b200va_devinfo_t* di, int resident, 
     return B200VA_OK;
 }
 
-// Ticket counters of the dynamic tile scheduler for direct launches: a ring of kSchedSlots two-word
-// slots per device, zeroed once and handed out round-robin, one per launch; the kernel's last CTA
-// zeroes its slot again (b200va_ptx.cuh: sched_retire).  Launches on one stream are ordered (every
-// counter access follows griddepcontrol.wait), so a slot is only ever shared by direct launches that
-// are kSchedSlots apart in issue order and run concurrently on different streams.  A captured graph
-// would keep its slots for every replay while the ring moves on and hands them to other launches,
-// so a loop handle's graph takes its counters from the handle instead (b200va_loop::ctr).
-constexpr unsigned kSchedSlots = 4096;
+// Ticket counters of the dynamic tile scheduler, two words each; the kernel's last CTA zeroes its
+// counter again (b200va_ptx.cuh: sched_retire).
+//  - Direct launches: a ring of kSchedSlots counters per device, handed out round-robin, one per
+//    launch.  Launches on one stream are ordered (every counter access follows griddepcontrol.wait),
+//    so a counter is only ever shared by direct launches that are kSchedSlots apart in issue order and
+//    run concurrently on different streams.
+//  - Launches captured into the caller's graph: the graph keeps its counter for every replay, so the
+//    counter comes from a separate pool of kCaptureSlots that direct launches never use, and the graph
+//    holds it for as long as it or an executable instance of it lives (a CUDA user object retained by
+//    the graph; its destructor puts the counter back).  An empty pool is an error, never a shared
+//    counter.  The executable instances of one graph share its counters: they must not run at once.
+//  - A loop handle's graph takes its counters from the handle (b200va_loop::ctr).
+constexpr unsigned kSchedSlots = 4096, kCaptureSlots = 16384;
 
 struct SchedPool {
-    std::once_flag once;
-    int rc = B200VA_OK;
-    unsigned int* ctr = nullptr;
+    std::mutex mu;
+    std::atomic<unsigned int*> ctr{nullptr};   // kSchedSlots ring counters, then kCaptureSlots capture counters
     std::atomic<unsigned> next{0};
+    std::vector<unsigned> free;                // capture counters no graph holds (under mu; capacity kCaptureSlots)
 };
 SchedPool g_sched[kMaxDevices];
 
-int sched_slot(int device, unsigned int** out)
+// Allocates and zeroes the device's counters on first use.  It may be the first call of a process and be made
+// inside the caller's stream capture, of any mode: the calling thread is switched to relaxed capture mode for the
+// allocation, which a global or thread-local capture prohibits, and the zeroing runs on a private stream.  A
+// failure is returned and not kept: the next call tries again.
+int sched_init(SchedPool& p)
+{
+    std::lock_guard<std::mutex> lk(p.mu);
+    if (p.ctr.load(std::memory_order_relaxed)) return B200VA_OK;
+    try {
+        p.free.reserve(kCaptureSlots);
+    } catch (...) {
+        return B200VA_ERR_NOMEM;
+    }
+    const size_t bytes = size_t{kSchedSlots + kCaptureSlots} * 2 * sizeof(unsigned int);
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    CU_TRY(cudaThreadExchangeStreamCaptureMode(&mode));
+    void* d = nullptr;
+    cudaStream_t st = nullptr;
+    cudaError_t e = cudaMalloc(&d, bytes);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d, 0, bytes, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (st) cudaStreamDestroy(st);
+    if (e != cudaSuccess && d) cudaFree(d);
+    cudaThreadExchangeStreamCaptureMode(&mode);            // the caller's mode again
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return cuda_err(e);
+    }
+    p.free.clear();
+    for (unsigned i = kCaptureSlots; i-- > 0;) p.free.push_back(i);
+    p.ctr.store(static_cast<unsigned int*>(d), std::memory_order_release);
+    return B200VA_OK;
+}
+
+struct HeldSlot {
+    SchedPool* pool;
+    unsigned slot;
+};
+
+// The user object's destructor: the graph and every executable instance of it are gone, and their launches have
+// completed.  Makes no CUDA call.
+void CUDART_CB release_slot(void* arg)
+{
+    HeldSlot* h = static_cast<HeldSlot*>(arg);
+    {
+        std::lock_guard<std::mutex> lk(h->pool->mu);
+        h->pool->free.push_back(h->slot);                  // within the reserved capacity: never allocates
+    }
+    delete h;
+}
+
+// A capture counter for a launch being captured into `graph`, held by the graph.
+int capture_slot(SchedPool& p, cudaGraph_t graph, unsigned int** out)
+{
+    HeldSlot* h = new (std::nothrow) HeldSlot{&p, 0};
+    if (!h) return B200VA_ERR_NOMEM;
+    {
+        std::lock_guard<std::mutex> lk(p.mu);
+        if (p.free.empty()) {
+            delete h;
+            return B200VA_ERR_NOMEM;
+        }
+        h->slot = p.free.back();
+        p.free.pop_back();
+    }
+    cudaUserObject_t obj = nullptr;
+    cudaError_t e = cudaUserObjectCreate(&obj, h, release_slot, 1, cudaUserObjectNoDestructorSync);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        release_slot(h);
+        return cuda_err(e);
+    }
+    e = cudaGraphRetainUserObject(graph, obj, 1, cudaGraphUserObjectMove);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        cudaUserObjectRelease(obj, 1);                     // runs release_slot
+        return cuda_err(e);
+    }
+    *out = p.ctr.load(std::memory_order_relaxed) + 2 * (kSchedSlots + h->slot);
+    return B200VA_OK;
+}
+
+// The counter of a dynamically scheduled launch on `stream`: a ring slot, or a capture counter if the stream is
+// capturing.
+int sched_slot(int device, cudaStream_t stream, unsigned int** out)
 {
     SchedPool& p = g_sched[device];
-    std::call_once(p.once, [&] {
-        void* d = nullptr;
-        cudaError_t e = cudaMalloc(&d, size_t{kSchedSlots} * 2 * sizeof(unsigned int));
-        if (e == cudaSuccess) e = cudaMemset(d, 0, size_t{kSchedSlots} * 2 * sizeof(unsigned int));
-        if (e != cudaSuccess) { cudaGetLastError(); if (d) cudaFree(d); p.rc = cuda_err(e); return; }
-        p.ctr = static_cast<unsigned int*>(d);
-    });
-    if (p.rc != B200VA_OK) return p.rc;
-    *out = p.ctr + 2 * (p.next.fetch_add(1, std::memory_order_relaxed) % kSchedSlots);
+    if (!p.ctr.load(std::memory_order_acquire)) RC_TRY(sched_init(p));
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    cudaGraph_t graph = nullptr;
+    const cudaError_t e = cudaStreamGetCaptureInfo(stream, &cs, nullptr, &graph);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return cuda_err(e);
+    }
+    if (cs == cudaStreamCaptureStatusActive) return capture_slot(p, graph, out);
+    if (cs != cudaStreamCaptureStatusNone) return cuda_err(cudaErrorStreamCaptureInvalidated);
+    *out = p.ctr.load(std::memory_order_relaxed) + 2 * (p.next.fetch_add(1, std::memory_order_relaxed) % kSchedSlots);
     return B200VA_OK;
 }
 
@@ -476,7 +569,7 @@ int b200va::launch(const float* dA, const float* dB, float* dC, size_t n, const 
     if (n == 0) return B200VA_OK;
     Plan p;
     RC_TRY(plan_launch(t, di, dA, dB, dC, n, &p));
-    if (p.ctr && !ctr) RC_TRY(sched_slot(di->device, &ctr));
+    if (p.ctr && !ctr) RC_TRY(sched_slot(di->device, stream, &ctr));
     const uint32_t tile = static_cast<uint32_t>(t.tile_bytes), stages = static_cast<uint32_t>(t.stages);
     switch (p.form) {
         case Form::Scalar:   // the control keeps the sample's plain launch (no programmatic dependent launch)
@@ -684,6 +777,10 @@ int b200va_add_f32_loop(const float* dA, const float* dB, float* dC, size_t n, i
         default_tune(variant, n, &t);
         return launch_chain(dA, dB, dC, n, t, false, iters, st, pdl_enabled());
     }
+    // the graph form creates a handle and drains the stream: refused before it touches a capturing stream
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    CU_TRY(cudaStreamIsCapturing(st, &cs));
+    if (cs != cudaStreamCaptureStatusNone) return cuda_err(cudaErrorStreamCaptureUnsupported);
     b200va_loop_t* l = nullptr;
     RC_TRY(b200va_loop_create(&l, dA, dB, dC, n, variant, graph_batch));
     int rc = b200va_loop_run(l, iters, stream);

@@ -69,7 +69,7 @@ const char* b200va_strerror(int code)
         case B200VA_ERR_VARIANT:   return "unknown kernel variant or unsupported geometry";
         case B200VA_ERR_NO_DEVICE: return "no sm_90 CUDA device";
         case B200VA_ERR_VERIFY:    return "result verification failed";
-        case B200VA_ERR_NOMEM:     return "host allocation failed";
+        case B200VA_ERR_NOMEM:     return "host allocation failed, or no captured-launch counter left";
     }
     if (code <= B200VA_ERR_CUDA_BASE) return cudaGetErrorString(static_cast<cudaError_t>(-code - 1000));
     return "unknown error";

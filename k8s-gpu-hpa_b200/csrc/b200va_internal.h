@@ -26,10 +26,14 @@ constexpr int kMaxDevices = 64;
 
 inline int cuda_err(cudaError_t e) { return e == cudaSuccess ? B200VA_OK : -(1000 + static_cast<int>(e)); }
 
+// A failure is returned, and not left latched as the runtime's last error for the caller's next launch check.
 #define CU_TRY(expr)                                   \
     do {                                               \
         cudaError_t e__ = (expr);                      \
-        if (e__ != cudaSuccess) return cuda_err(e__);  \
+        if (e__ != cudaSuccess) {                      \
+            cudaGetLastError();                        \
+            return cuda_err(e__);                      \
+        }                                              \
     } while (0)
 
 #define RC_TRY(expr)                   \
@@ -148,7 +152,8 @@ inline int check_convert_operands(size_t esa, const void* pa, size_t esc, const 
 void default_tune(int variant, size_t n, b200va_tune_t* t, unsigned flags = 0);
 int check_variant(int variant, unsigned flags = 0);
 // `ctr`: the dynamic tile scheduler's two-word ticket counter (zeroed; the kernel leaves it zeroed
-// again); nullptr takes the next slot of the device's ring.
+// again); nullptr takes the next slot of the device's ring, or, when `stream` is capturing, a counter
+// the captured graph holds until it is destroyed.
 int launch(const float* dA, const float* dB, float* dC, size_t n, const b200va_tune_t& t, cudaStream_t stream, bool pdl,
            unsigned int* ctr = nullptr);
 
