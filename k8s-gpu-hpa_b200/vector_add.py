@@ -38,6 +38,20 @@ def _dev_ptr(t, name: str) -> int:
     return t.data_ptr()
 
 
+def _f32_operands(ref: str, **operands) -> tuple[int, ...]:
+    """The device pointers of the operands, in order, each checked by _dev_ptr and all checked to have the length of
+    operand `ref` and to lie on its device, before the caller makes any C-ABI call (a shorter operand would be read or
+    written past its end)."""
+    ptrs = tuple(_dev_ptr(t, name) for name, t in operands.items())
+    r = operands[ref]
+    for name, t in operands.items():
+        if t.numel() != r.numel():
+            raise ValueError(f"{name} differs from {ref} in length ({t.numel()} elements, {ref} has {r.numel()})")
+        if t.device != r.device:
+            raise ValueError(f"{name} is on {t.device}, {ref} on {r.device}")
+    return ptrs
+
+
 def _stream_ptr(stream) -> int:
     torch = _torch()
     if stream is None:
@@ -53,13 +67,9 @@ def add(a, b, out=None, *, variant=K_AUTO, tune: Tune | None = None, stream=None
     libb200va_tune.so, which carries every geometry (the production library refuses the
     ones AUTO never picks with ERR_VARIANT)."""
     torch = _torch()
-    if a.numel() != b.numel():
-        raise ValueError("a and b differ in length")
     if out is None:
         out = torch.empty_like(a)
-    if out.numel() != a.numel():
-        raise ValueError("out differs in length")
-    pa, pb, pc = _dev_ptr(a, "a"), _dev_ptr(b, "b"), _dev_ptr(out, "out")
+    pa, pb, pc = _f32_operands("a", a=a, b=b, out=out)
     with torch.cuda.device(a.device):
         if tune is not None:
             h = capi.tune_lib() if full_matrix else lib
@@ -75,7 +85,7 @@ def add(a, b, out=None, *, variant=K_AUTO, tune: Tune | None = None, stream=None
 def add_loop(a, b, out, iters: int, *, graph_batch: int = 0, variant=K_AUTO, stream=None):
     """The launch loop in-process: ``iters`` launches (CUDA-graph batched if graph_batch>1)."""
     torch = _torch()
-    pa, pb, pc = _dev_ptr(a, "a"), _dev_ptr(b, "b"), _dev_ptr(out, "out")
+    pa, pb, pc = _f32_operands("a", a=a, b=b, out=out)
     with torch.cuda.device(a.device):
         check(lib.b200va_add_f32_loop(pa, pb, pc, a.numel(), _variant(variant), iters, graph_batch,
                                       _stream_ptr(stream)), "b200va_add_f32_loop")
@@ -89,11 +99,12 @@ class Loop:
     def __init__(self, a, b, out, *, graph_batch: int = 50, variant=K_AUTO):
         torch = _torch()
         self._h = C.c_void_p()
+        pa, pb, pc = _f32_operands("a", a=a, b=b, out=out)
         self._keep = (a, b, out)
         self._device = a.device
         with torch.cuda.device(a.device):
-            check(lib.b200va_loop_create(C.byref(self._h), _dev_ptr(a, "a"), _dev_ptr(b, "b"), _dev_ptr(out, "out"), a.numel(),
-                                         _variant(variant), graph_batch), "b200va_loop_create")
+            check(lib.b200va_loop_create(C.byref(self._h), pa, pb, pc, a.numel(), _variant(variant), graph_batch),
+                  "b200va_loop_create")
 
     def run(self, iters: int, *, stream=None) -> None:
         torch = _torch()
@@ -360,11 +371,16 @@ def dot(a, b, *, out=None, workspace=None, stream=None):
 
 
 def probe(kind: str, a, b, c, *, stream=None):
-    """Ceiling probe (b200va_probe_f32): 'read2' loads a and b, 'fill' stores c, 'copy' c = a.  c is clobbered."""
+    """Ceiling probe (b200va_probe_f32): 'read2' loads a and b, 'fill' stores c, 'copy' c = a.  c is clobbered.
+    The operands the kind uses are checked like add's (float32, contiguous, c's length on c's device); the others
+    are ignored."""
     torch = _torch()
+    code = capi.PROBES[kind]
+    used = {"a": a, "b": b} if kind == "read2" else {"a": a} if kind == "copy" else {}
+    *_, pc = _f32_operands("c", **used, c=c)
+    pa, pb = (used[k].data_ptr() if k in used else None for k in ("a", "b"))
     with torch.cuda.device(c.device):
-        check(lib.b200va_probe_f32(capi.PROBES[kind], a.data_ptr() if a is not None else None, b.data_ptr() if b is not None else None,
-                                   _dev_ptr(c, "c"), c.numel(), _stream_ptr(stream)), "b200va_probe_f32")
+        check(lib.b200va_probe_f32(code, pa, pb, pc, c.numel(), _stream_ptr(stream)), "b200va_probe_f32")
 
 
 def fill_ctr(out, seed: int, first: int = 0, *, stream=None):
@@ -392,10 +408,10 @@ def fill_rand_host(n: int) -> tuple[np.ndarray, np.ndarray]:
 def verify(a, b, c, *, stream=None) -> tuple[int, int]:
     """Device-side bitwise check; returns (mismatch count, first bad index or -1). Synchronises."""
     torch = _torch()
+    pa, pb, pc = _f32_operands("a", a=a, b=b, c=c)
     res = torch.empty(2, dtype=torch.int64, device=a.device)
     with torch.cuda.device(a.device):
-        check(lib.b200va_verify_f32(_dev_ptr(a, "a"), _dev_ptr(b, "b"), _dev_ptr(c, "c"), a.numel(),
-                                    res.data_ptr(), _stream_ptr(stream)), "b200va_verify_f32")
+        check(lib.b200va_verify_f32(pa, pb, pc, a.numel(), res.data_ptr(), _stream_ptr(stream)), "b200va_verify_f32")
     bad, first = (int(v) & 0xFFFFFFFFFFFFFFFF for v in res.tolist())
     return bad, (-1 if bad == 0 else first)
 
