@@ -323,6 +323,36 @@ int b200va_quantize_fp8(int src_dtype, const void *dA, int fp8, void *dC, size_t
                         int scale_exp, double *d_amax, void *stream);
 int b200va_dequantize_fp8(int fp8, const void *dA, int dst_dtype, void *dC, size_t n,
                           int scale_exp, void *stream);
+/* The same casts with the scale exponent k in device memory, chosen there from the tensor's amax ("current
+ * scaling"), or from a running amax the caller keeps in *d_amax, with no host read between the passes.
+ * Quantize is two launches on `stream`:
+ *   1. Amax pass: *d_amax = max(*d_amax, M), M the largest FINITE |a_i| widened exactly to f64 (0 when there is
+ *      none).  NaN and +-inf do not take part: this is the MXFP8 block-maximum rule, not the NaN-propagating amax of
+ *      b200va_quantize_fp8.  One atomic per CTA on the f64 bits, so it is exact and independent of order.  Set
+ *      *d_amax = +0.0 before the call for current scaling; left as it is, the scale follows the running max.
+ *   2. Scale: from the value m in *d_amax after the amax pass, K(m) is the largest integer k with
+ *      m * 2^k <= max finite (448 / 57344), K(0) = +inf; with emax = 8 (E4M3) / 15 (E5M2) it reads off the bits as
+ *      K = emax - floor(log2 m) - (m * 2^-floor(log2 m) > 1.75), the negated B200VA_MX_SCALE_NOSAT exponent.
+ *      k = clamp(K(m) - margin, -126, 126); k = 0 if *d_amax does not hold +0.0 or a positive finite value, which
+ *      happens only when the caller left a NaN, +inf or a value with the sign bit set (-0.0 included) there: the
+ *      amax pass's maximum is taken on the bit patterns as unsigned integers, so it keeps those.  Every CTA computes k
+ *      once the amax pass has completed; one thread writes it to *d_scale_exp.
+ *   3. Quantize: c[i] = sat(RN(a[i] * 2^k)) by exactly the rules of b200va_quantize_fp8.  With margin >= 0 and k not
+ *      clamped, no finite element saturates (|a_i| * 2^k <= max finite); only +-inf does.
+ * Dequantize is one launch: c[i] = a[i] * 2^-k rounded once by b200va_dequantize_fp8's rules, k read from
+ * *d_scale_exp once the launch before it has completed.  A k outside [-126, 126] makes every element a NaN (the
+ * device-side counterpart of the E8M0 0xFF rule: the host cannot check a value that lives on the device).
+ * 2^-k in f32 is the per-tensor dequantization scale an FP8 GEMM takes from a device tensor.
+ * margin lies in [0, 126]; d_amax is 8-byte and d_scale_exp 4-byte aligned, both non-NULL.
+ * B200VA_ERR_VARIANT: bad dtype or FP8 code.  B200VA_ERR_INVALID: margin out of range, NULL d_amax or d_scale_exp,
+ * NULL dA/dC with n > 0, n > 2^40.  B200VA_ERR_ALIGN: dA/dC not aligned to their element size, d_amax or d_scale_exp
+ * misaligned.  B200VA_ERR_OVERLAP: C meets A, or d_amax (quantize) or d_scale_exp meets A, C or the other.  A
+ * rejected call writes nothing; n = 0 writes nothing and launches nothing (*d_scale_exp keeps its value).
+ * Asynchronous on `stream`: no allocation, synchronisation or memset; capturable in a CUDA graph. */
+int b200va_quantize_fp8_auto(int src_dtype, const void *dA, int fp8, void *dC, size_t n,
+                             int margin, double *d_amax, int32_t *d_scale_exp, void *stream);
+int b200va_dequantize_fp8_auto(int fp8, const void *dA, int dst_dtype, void *dC, size_t n,
+                               const int32_t *d_scale_exp, void *stream);
 
 /* ---- block-scaled FP8 (MXFP8) quantize and dequantize (row f4) --------------------------------
  * The same two FP8 formats with one scale per block of `block` elements, block one of 32 (OCP Microscaling MXFP8),

@@ -5,7 +5,14 @@
 //   dequantize  c[i] = RN(a[i] 2^-k)       rounded once to the destination, overflow to +-inf
 //
 // One kernel per non-FP8 type, fp8_quant_vec<SRC> and fp8_dequant_vec<DST>, each carrying a body per format that a
-// uniform argument picks at the top (16 pairs in 8 kernels).  How one rounding is reached:
+// uniform argument picks at the top (16 pairs in 8 kernels).  The same kernels carry b200va_quantize_fp8_auto and
+// b200va_dequantize_fp8_auto, whose scale exponent k lives in device memory:
+//   amax pass   fp8_quant_vec with C = nullptr: the largest finite |a_i| max-accumulated into *amax, nothing stored
+//   quantize    fp8_quant_vec with amax_in: k = auto_scale_exp(*amax_in), read after the dependency wait, and
+//               written to *k_out by one thread
+//   dequantize  fp8_dequant_vec with k_in: k = *k_in, read after the dependency wait; outside [-126, 126] the
+//               scale is a NaN
+// How one rounding is reached:
 // - f32, f16, bf16 sources widen exactly to f32 and are scaled there; cvt.rn.satfinite.{e4m3x2,e5m2x2}.f32 rounds.
 //   Where the f32 product is inexact (below 2^-126) the exact value lies far below half the smallest FP8
 //   subnormal, so the result is +-0 either way; where it overflows, the exact value saturates either way.
@@ -80,6 +87,33 @@ __device__ __forceinline__ float f32_round_odd(double x)
 // keeps the order) and as f64 bits for f64.  Every NaN pattern sorts above +inf.
 template <int SRC>
 using amax_bits_t = std::conditional_t<SRC == DT_F64, unsigned long long, uint32_t>;
+
+// The magnitude bit pattern of element e of the source words s if it is finite, else 0 (NaN and +-inf do not take
+// part in a finite maximum): f32 bits for the f32 family, f64 bits for f64, as amax_bits_t.
+template <int SRC>
+__device__ __forceinline__ amax_bits_t<SRC> finite_mag(const uint32_t* s, int e)
+{
+    if constexpr (SRC == DT_F64) {
+        const unsigned long long v = static_cast<unsigned long long>(__double_as_longlong(elem_f64(s, e))) & 0x7fffffffffffffffull;
+        return v < 0x7ff0000000000000ull ? v : 0ull;
+    } else {
+        const uint32_t v = __float_as_uint(elem_f32<SRC>(s, e)) & 0x7fffffffu;
+        return v < 0x7f800000u ? v : 0u;
+    }
+}
+
+// The scale exponent b200va_quantize_fp8_auto takes from the value m its amax pass left: with m = s 2^e (s in
+// [1, 2)), K = emax - e - (s > 1.75) is the largest k with m 2^k <= max finite = 1.75 2^emax, and k = K - margin
+// clamped to [-126, 126].  An f64 subnormal m or m = +0 reads as e = -1023, which clamps to 126 as K(0) = +inf
+// does.  m whose pattern is not that of a finite value with the sign bit clear (a NaN, +inf, or a negative value
+// or -0.0 the caller left, which the amax pass's unsigned maximum keeps) gives 0.
+__device__ __forceinline__ int auto_scale_exp(double m, int fmt, int margin)
+{
+    const unsigned long long b = static_cast<unsigned long long>(__double_as_longlong(m));
+    if (b >= 0x7ff0000000000000ull) return 0;
+    const int K = (fmt == F8_E4M3 ? 8 : 15) - (static_cast<int>(b >> 52) - 1023) - ((b & 0x000fffffffffffffull) > 0x000c000000000000ull);
+    return min(max(K - margin, -126), 126);
+}
 
 // Elements e0 and e0 + 1 of the source words s, scaled by 2^k and rounded to two FP8 bytes (bits 0..15); m takes
 // their magnitudes.  With `one`, only e0 (the high byte is 0).
@@ -165,12 +199,37 @@ __device__ __forceinline__ void quant_body(const unsigned char* a, unsigned char
     cast_edges(n, head, head + ngroups * 16, [&](size_t e) { c[e] = quant_elem<SRC, F8>(a + e * ES, k, m); });
 }
 
+// The amax pass's body after the dependency wait: quant_body's tiles and edges over A alone (elements [head, head +
+// 16 ngroups) on 16-byte boundaries in A), each element's finite magnitude folded into m and nothing stored.
+template <int SRC>
+__device__ __forceinline__ void amax_body(const unsigned char* a, size_t n, size_t head, size_t ngroups, int unroll,
+                                          amax_bits_t<SRC>& m)
+{
+    constexpr int ES = dt_traits<SRC>::size;
+    const unsigned char* ab = a + head * ES;
+    cast_tiles(unroll, ngroups, [=](size_t g) { return ld_vecs<ES>(ab, g); }, [&](size_t, const vecs<ES>& in) {
+        uint32_t s[4 * ES];
+        unpack<ES>(in.v, s);
+#pragma unroll
+        for (int e = 0; e < 16; ++e) m = max(m, finite_mag<SRC>(s, e));
+    });
+    cast_edges(n, head, head + ngroups * 16, [&](size_t e) {
+        uint32_t s[2];
+        ld_elem<ES>(a + e * ES, s);
+        m = max(m, finite_mag<SRC>(s, 0));
+    });
+}
+
 // One kernel per source type, the format picking one of its two bodies (with_f8).  unroll (1 or 2) and prefetch_first
 // are the launch's geometry, as in convert_vec.  With amax, each CTA max-accumulates its largest |a_i| (as f64 bits)
-// into *amax with one atomic, after the dependency wait like every other access.
+// into *amax with one atomic, after the dependency wait like every other access; both bodies reach that one atomic.
+// Without C the kernel is b200va_quantize_fp8_auto's amax pass (amax_body: finite magnitudes only, fmt and k unused).
+// With amax_in, k is auto_scale_exp(*amax_in, fmt, margin) instead of the argument, and thread 0 of CTA 0 writes it
+// to *k_out.
 template <int SRC>
 __global__ void fp8_quant_vec(const void* A, void* C, size_t n, size_t head, size_t ngroups, int unroll,
-                              int prefetch_first, int fmt, int k, double* amax)
+                              int prefetch_first, int fmt, int k, double* amax, const double* amax_in, int margin,
+                              int32_t* k_out)
 {
     const unsigned char* a = static_cast<const unsigned char*>(A);
     unsigned char* c = static_cast<unsigned char*>(C);
@@ -178,7 +237,15 @@ __global__ void fp8_quant_vec(const void* A, void* C, size_t n, size_t head, siz
     pdl_wait();
 
     amax_bits_t<SRC> m = 0;
-    with_f8(fmt, [&](auto F8) { quant_body<SRC, F8>(a, c, n, head, ngroups, unroll, k, m); });
+    if (!c) {
+        amax_body<SRC>(a, n, head, ngroups, unroll, m);
+    } else {
+        if (amax_in) {
+            k = auto_scale_exp(*amax_in, fmt, margin);
+            if (blockIdx.x == 0 && threadIdx.x == 0) *k_out = k;
+        }
+        with_f8(fmt, [&](auto F8) { quant_body<SRC, F8>(a, c, n, head, ngroups, unroll, k, m); });
+    }
     if (amax) cta_amax<SRC>(amax, m);
 }
 
@@ -237,19 +304,25 @@ __device__ __forceinline__ void dequant_body(const unsigned char* a, unsigned ch
 }
 
 // One kernel per destination type, the format picked at the top as in fp8_quant_vec; every slice has the scale 2^-k.
+// With k_in, k is *k_in, read once per thread after the dependency wait, and a k outside [-126, 126] scales by a NaN.
 template <int DST>
 __global__ void fp8_dequant_vec(const void* A, void* C, size_t n, size_t head, size_t ngroups, int unroll,
-                                int prefetch_first, int fmt, int k)
+                                int prefetch_first, int fmt, int k, const int32_t* k_in)
 {
+    using S = typename dt_traits<DST>::scalar;
     constexpr int ES = dt_traits<DST>::size;
     const unsigned char* a = static_cast<const unsigned char*>(A);
     unsigned char* c = static_cast<unsigned char*>(C);
     prefetch_first_tile<16 / ES, 1>(prefetch_first, a, head, ngroups * ES, unroll);
     pdl_wait();
 
-    with_f8(fmt, [=](auto F8) {
-        dequant_body<F8, DST>(a, c, n, head, ngroups, unroll, [=](size_t) { return pow2<DST>(-k); });
-    });
+    S s = pow2<DST>(-k);
+    if (k_in) {
+        const int kd = *k_in;
+        if constexpr (DST == DT_F64) s = kd >= -126 && kd <= 126 ? pow2<DST>(-kd) : __longlong_as_double(0x7ff8000000000000ll);
+        else s = kd >= -126 && kd <= 126 ? pow2<DST>(-kd) : __uint_as_float(0x7fc00000u);
+    }
+    with_f8(fmt, [=](auto F8) { dequant_body<F8, DST>(a, c, n, head, ngroups, unroll, [=](size_t) { return s; }); });
 }
 
 }  // namespace b200va

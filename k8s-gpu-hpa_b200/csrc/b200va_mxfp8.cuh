@@ -47,20 +47,6 @@ namespace b200va {
 
 enum : int { MX_SCALE_OCP = 0, MX_SCALE_NOSAT = 1, MX_SCALE_COUNT = 2 };
 
-// The magnitude bit pattern of element e of the source words s if it is finite, else 0 (NaN and +-inf do not take
-// part in a block's maximum): f32 bits for the f32 family, f64 bits for f64, as amax_bits_t.
-template <int SRC>
-__device__ __forceinline__ amax_bits_t<SRC> finite_mag(const uint32_t* s, int e)
-{
-    if constexpr (SRC == DT_F64) {
-        const unsigned long long v = static_cast<unsigned long long>(__double_as_longlong(elem_f64(s, e))) & 0x7fffffffffffffffull;
-        return v < 0x7ff0000000000000ull ? v : 0ull;
-    } else {
-        const uint32_t v = __float_as_uint(elem_f32<SRC>(s, e)) & 0x7fffffffu;
-        return v < 0x7f800000u ? v : 0u;
-    }
-}
-
 // The block's scale exponent e from its finite maximum m (see "The exponent" above).
 template <int SRC, int F8>
 __device__ __forceinline__ int mx_exponent(amax_bits_t<SRC> m, int rule)

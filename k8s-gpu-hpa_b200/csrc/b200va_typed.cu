@@ -167,19 +167,36 @@ int launch_convert_typed(const void* dA, void* dC, size_t n, cudaStream_t st)
 
 // b200va_quantize_fp8 (QUANT: T -> fmt) and b200va_dequantize_fp8 (fmt -> T): one fp8_quant_vec<T> or
 // fp8_dequant_vec<T> launch, the format passed to the kernel.  A unit is a group of 16 when quantizing and a 16-byte
-// output slice (sizeof T per group) when dequantizing.
+// output slice (sizeof T per group) when dequantizing.  The _auto forms pass the device-side k: quantize reads the
+// amax at amax_in and writes k to *scale_exp, dequantize reads k from *scale_exp.
 template <bool QUANT, int T>
-int launch_fp8_typed(const void* dA, void* dC, size_t n, int fmt, int k, double* amax, cudaStream_t st)
+int launch_fp8_typed(const void* dA, void* dC, size_t n, int fmt, int k, double* amax, cudaStream_t st,
+                     const double* amax_in = nullptr, int margin = 0, int32_t* scale_exp = nullptr)
 {
     constexpr size_t ES = dt_traits<T>::size;
     const cast_plan p = plan_cast(reinterpret_cast<uintptr_t>(dA), QUANT ? ES : 1, reinterpret_cast<uintptr_t>(dC),
                                   QUANT ? 1 : ES, n, QUANT ? 1 : ES);
     if constexpr (QUANT)
         return launch_kernel(fp8_quant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
-                             p.unroll, p.prefetch_first, fmt, k, amax);
+                             p.unroll, p.prefetch_first, fmt, k, amax, amax_in, margin, scale_exp);
     else
         return launch_kernel(fp8_dequant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
-                             p.unroll, p.prefetch_first, fmt, k);
+                             p.unroll, p.prefetch_first, fmt, k, static_cast<const int32_t*>(scale_exp));
+}
+
+// b200va_quantize_fp8_auto's amax pass: one fp8_quant_vec<T> launch without C.  There is no C to share a phase with,
+// so the vector body starts at the head that puts A alone on a 16-byte boundary; a unit is a group of 16, and every
+// element outside the body an edge item.  The geometry follows A's HBM class.
+template <int T>
+int launch_fp8_amax(const void* dA, size_t n, double* amax, cudaStream_t st)
+{
+    constexpr size_t ES = dt_traits<T>::size;
+    cast_plan p{};
+    p.head = std::min(head_peel(reinterpret_cast<uintptr_t>(dA), ES), n);
+    p.ngroups = (n - p.head) / 16;
+    plan_geometry(p, hbm_class(n, ES), p.ngroups, n - p.ngroups * 16);
+    return launch_kernel(fp8_quant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, nullptr, n, p.head, p.ngroups,
+                         p.unroll, p.prefetch_first, 0, 0, amax, nullptr, 0, nullptr);
 }
 
 // The argument rules the two FP8 entry points share, after the dtype and format codes: scale_exp in [-126, 126],
@@ -191,6 +208,18 @@ int check_fp8_args(size_t es, const void* dA, size_t esc, const void* dC, size_t
     RC_TRY(check_convert_operands(es, dA, esc, dC, n));
     if (reinterpret_cast<uintptr_t>(d_amax) & 7u) return B200VA_ERR_ALIGN;
     if (d_amax && (ranges_meet(d_amax, 8, dA, n * es) || ranges_meet(d_amax, 8, dC, n * esc)))
+        return B200VA_ERR_OVERLAP;
+    return B200VA_OK;
+}
+
+// What the two _auto entry points check after check_fp8_args: d_scale_exp (non-NULL) 4-byte aligned and meeting
+// neither A, C nor d_amax (NULL for dequantize).
+int check_scale_exp_arg(size_t es, const void* dA, size_t esc, const void* dC, size_t n, const double* d_amax,
+                        const int32_t* d_scale_exp)
+{
+    if (reinterpret_cast<uintptr_t>(d_scale_exp) & 3u) return B200VA_ERR_ALIGN;
+    if (ranges_meet(d_scale_exp, 4, dA, n * es) || ranges_meet(d_scale_exp, 4, dC, n * esc) ||
+        ranges_meet(d_scale_exp, 4, d_amax, d_amax ? 8 : 0))
         return B200VA_ERR_OVERLAP;
     return B200VA_OK;
 }
@@ -302,6 +331,43 @@ int b200va_dequantize_fp8(int fp8, const void* dA, int dst_dtype, void* dC, size
     int rc = B200VA_ERR_VARIANT;
     with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dst_dtype, [&](auto DST) {
         rc = launch_fp8_typed<false, DST>(dA, dC, n, fp8, scale_exp, nullptr, static_cast<cudaStream_t>(stream));
+    });
+    return rc;
+}
+
+int b200va_quantize_fp8_auto(int src_dtype, const void* dA, int fp8, void* dC, size_t n, int margin, double* d_amax,
+                             int32_t* d_scale_exp, void* stream)
+{
+    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    if (margin < 0 || margin > 126 || !d_amax || !d_scale_exp) return B200VA_ERR_INVALID;
+    const size_t es = dtype_size(src_dtype);
+    RC_TRY(check_fp8_args(es, dA, 1, dC, n, 0, d_amax));
+    RC_TRY(check_scale_exp_arg(es, dA, 1, dC, n, d_amax, d_scale_exp));
+    if (n == 0) return B200VA_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int rc = B200VA_ERR_VARIANT;
+    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(src_dtype, [&](auto SRC) {
+        rc = launch_fp8_amax<SRC>(dA, n, d_amax, st);
+        if (rc == B200VA_OK) rc = launch_fp8_typed<true, SRC>(dA, dC, n, fp8, 0, nullptr, st, d_amax, margin, d_scale_exp);
+    });
+    return rc;
+}
+
+int b200va_dequantize_fp8_auto(int fp8, const void* dA, int dst_dtype, void* dC, size_t n, const int32_t* d_scale_exp,
+                               void* stream)
+{
+    if (dst_dtype < 0 || dst_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    if (!d_scale_exp) return B200VA_ERR_INVALID;
+    const size_t es = dtype_size(dst_dtype);
+    RC_TRY(check_fp8_args(1, dA, es, dC, n, 0, nullptr));
+    RC_TRY(check_scale_exp_arg(1, dA, es, dC, n, nullptr, d_scale_exp));
+    if (n == 0) return B200VA_OK;
+    int rc = B200VA_ERR_VARIANT;
+    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dst_dtype, [&](auto DST) {
+        rc = launch_fp8_typed<false, DST>(dA, dC, n, fp8, 0, nullptr, static_cast<cudaStream_t>(stream), nullptr, 0,
+                                          const_cast<int32_t*>(d_scale_exp));
     });
     return rc;
 }

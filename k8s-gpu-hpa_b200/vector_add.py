@@ -235,6 +235,57 @@ def dequantize_fp8(a, dtype, *, scale_exp: int = 0, out=None, stream=None):
     return out
 
 
+def _one_element(t, dtype, a, name: str):
+    """``t`` checked to be a one-element tensor of ``dtype`` on a's device."""
+    torch = _torch()
+    if not isinstance(t, torch.Tensor) or t.dtype != dtype or t.numel() != 1 or t.device != a.device:
+        raise TypeError(f"{name} must be a one-element {dtype} tensor on a's device")
+    return t
+
+
+def quantize_fp8_auto(a, fmt, *, margin: int = 0, amax=None, scale_exp=None, out=None, stream=None):
+    """``a`` (f32/f64/f16/bf16) quantized to FP8 with a power-of-two scale 2^k chosen on the device from the amax
+    (b200va_quantize_fp8_auto): an amax pass max-accumulates the largest finite |a| into ``amax``, then k is the
+    largest exponent with amax 2^k <= max finite (448 for E4M3, 57344 for E5M2), less ``margin`` (0..126), clamped to
+    [-126, 126], and a[i] 2^k is rounded once by quantize_fp8's rules.  With margin >= 0, only +-inf saturates.
+    ``amax``: a one-element float64 CUDA tensor, the caller's running max; None makes a zeroed one on the stream
+    (current scaling).  ``scale_exp``: a one-element int32 CUDA tensor that receives k, else a new one.  ``out``: as
+    in quantize_fp8.  Returns (out, scale_exp) without a host sync; torch.exp2(-scale_exp.float()) is the per-tensor
+    dequantization scale a tensor-wise torch._scaled_mm takes.  Asynchronous on the current stream."""
+    torch = _torch()
+    src = _operand(a, "a")
+    dtype, code = _fp8_format(fmt)
+    out = _out(out, dtype, a)
+    if amax is not None:
+        _one_element(amax, torch.float64, a, "amax")
+    scale_exp = (torch.empty(1, dtype=torch.int32, device=a.device) if scale_exp is None
+                 else _one_element(scale_exp, torch.int32, a, "scale_exp"))
+    with torch.cuda.device(a.device):
+        st = stream if stream is not None else torch.cuda.current_stream()
+        if amax is None:
+            with torch.cuda.stream(st):
+                amax = torch.zeros(1, dtype=torch.float64, device=a.device)
+        check(lib.b200va_quantize_fp8_auto(src, a.data_ptr(), code, out.data_ptr(), a.numel(), int(margin),
+                                           amax.data_ptr(), scale_exp.data_ptr(), st.cuda_stream),
+              "b200va_quantize_fp8_auto")
+    return out, scale_exp
+
+
+def dequantize_fp8_auto(q, scale_exp, dtype, *, out=None, stream=None):
+    """FP8 ``q`` times 2^-k, k the one-element int32 CUDA tensor ``scale_exp`` that quantize_fp8_auto wrote, rounded
+    once to ``dtype`` by dequantize_fp8's rules (b200va_dequantize_fp8_auto); k is read on the device, and one outside
+    [-126, 126] makes every element NaN.  ``out``: as in dequantize_fp8.  Asynchronous on the current stream."""
+    torch = _torch()
+    code = _operand(q, "q", _fp8_format)
+    dtype, dst = _float_dtype(dtype)
+    _one_element(scale_exp, torch.int32, q, "scale_exp")
+    out = _out(out, dtype, q)
+    with torch.cuda.device(q.device):
+        check(lib.b200va_dequantize_fp8_auto(code, q.data_ptr(), dst, out.data_ptr(), q.numel(), scale_exp.data_ptr(),
+                                             _stream_ptr(stream)), "b200va_dequantize_fp8_auto")
+    return out
+
+
 _U64 = (1 << 64) - 1
 
 

@@ -7,11 +7,15 @@ Per round, every op of the chosen families is timed at n elements with CUDA even
 and the algorithmic bytes of one call:
   convert  every ordered pair of distinct types of f32, f64, f16, bf16: n * (sizeof SRC + sizeof DST);
   fp8      per type and format (E4M3, E5M2): quantize without amax, quantize with amax, dequantize back:
-           n * (sizeof T + 1);
+           n * (sizeof T + 1); then the per-tensor scale taken from the amax, two ways: the two-pass recipe,
+           b200va_quantize_fp8 with amax into a scratch output (the pass that finds the scale) followed by the real
+           b200va_quantize_fp8, 2 n * (sizeof T + 1) bytes as it runs here (without the host read of the amax that
+           a caller needs between the two); and b200va_quantize_fp8_auto, its amax pass and the quantize with the
+           k chosen on the device, n * (2 sizeof T + 1).  "us" is the time of the whole recipe, "TB/s" counts what
+           it moves; neither resets the amax between calls (a running max).  Last, b200va_dequantize_fp8_auto with
+           the device k, n * (sizeof T + 1).
   mxfp8    per type and format, alternated in this order: quantize and dequantize at block 32 and at block 128,
-           n * (sizeof T + 1 + 1 / block); then the two-pass per-tensor recipe they replace, b200va_quantize_fp8 with
-           amax into a scratch output (the pass that finds the scale) followed by the real b200va_quantize_fp8,
-           2 n * (sizeof T + 1) bytes as it runs here ("us" is the time of the pair, "TB/s" counts what the pair moves).
+           n * (sizeof T + 1 + 1 / block); the per-tensor recipes they compete with are in the fp8 family.
   sr       the stochastically rounding casts from f32, each beside its round-to-nearest counterpart: to f16 and bf16,
            and to E4M3 and E5M2 without and with amax, n * (4 + sizeof DST); then the torch-eager bf16 recipe (a random
            int32 tensor as large as the input, added to the f32 patterns, masked and cast in separate kernels), counted
@@ -79,18 +83,27 @@ def fp8_ops(torch, va, n, tdt, f8):
             yield f"quantize {s}->{f}", lambda: va.quantize_fp8(a, f8[f], out=q), nbytes
             yield f"quantize {s}->{f} amax", lambda: va.quantize_fp8(a, f8[f], amax=amax, out=q), nbytes
             yield f"dequantize {f}->{s}", lambda: va.dequantize_fp8(q, tdt[s], out=c), nbytes
-            del q, c
+            scratch = torch.empty(n, dtype=f8[f], device="cuda")
+            k = torch.zeros(1, dtype=torch.int32, device="cuda")
+
+            def two_pass():
+                va.quantize_fp8(a, f8[f], amax=amax, out=scratch)
+                va.quantize_fp8(a, f8[f], out=q)
+
+            yield f"two-pass per-tensor quantize {s}->{f}", two_pass, 2 * n * (SIZE[s] + 1)
+            yield (f"quantize_fp8_auto {s}->{f}", lambda: va.quantize_fp8_auto(a, f8[f], amax=amax, scale_exp=k, out=q),
+                   n * (2 * SIZE[s] + 1))
+            yield f"dequantize_fp8_auto {f}->{s}", lambda: va.dequantize_fp8_auto(q, k, tdt[s], out=c), nbytes
+            del q, c, scratch, k
         del a, amax
 
 
 def mxfp8_ops(torch, va, n, tdt, f8):
     for s in tdt:
         a = torch.randn(n, dtype=torch.float32, device="cuda").to(tdt[s])
-        amax = torch.zeros(1, dtype=torch.float64, device="cuda")
         c = torch.empty(n, dtype=tdt[s], device="cuda")
         for f in f8:
             q = torch.empty(n, dtype=f8[f], device="cuda")
-            scratch = torch.empty(n, dtype=f8[f], device="cuda")
             for block in (32, 128):
                 sc = torch.empty(n // block, dtype=torch.uint8, device="cuda")
                 nbytes = n * (SIZE[s] + 1) + n // block
@@ -99,14 +112,8 @@ def mxfp8_ops(torch, va, n, tdt, f8):
                 yield (f"mx dequantize {f}->{s} block {block}",
                        lambda: va.dequantize_mxfp8(q, sc, tdt[s], block=block, out=c), nbytes)
                 del sc
-
-            def two_pass():
-                va.quantize_fp8(a, f8[f], amax=amax, out=scratch)
-                va.quantize_fp8(a, f8[f], out=q)
-
-            yield f"two-pass per-tensor quantize {s}->{f}", two_pass, 2 * n * (SIZE[s] + 1)
-            del q, scratch
-        del a, amax, c
+            del q
+        del a, c
 
 
 def sr_ops(torch, va, n, tdt, f8):
