@@ -353,6 +353,27 @@ int b200va_quantize_fp8_auto(int src_dtype, const void *dA, int fp8, void *dC, s
                              int margin, double *d_amax, int32_t *d_scale_exp, void *stream);
 int b200va_dequantize_fp8_auto(int fp8, const void *dA, int dst_dtype, void *dC, size_t n,
                                const int32_t *d_scale_exp, void *stream);
+/* Quantize-transpose: the FP8 bytes of a 2-D tensor and their transpose in one pass over it, the operands an H100
+ * FP8 GEMM takes K-major on both sides (the forward product uses C, the backward products Ct).  A is row-major
+ * rows x cols, contiguous (row stride cols); C is row-major rows x cols and Ct row-major cols x rows.  With
+ * n = rows * cols:
+ *   - C holds exactly the bytes b200va_quantize_fp8 (or b200va_quantize_fp8_auto) writes for n elements of A, and
+ *     Ct[j * rows + i] == C[i * cols + j].
+ *   - *d_amax ends with exactly the bits the 1-D call leaves: the NaN-propagating amax here (d_amax may be NULL),
+ *     the finite-only amax pass in the _auto form, which also writes k to *d_scale_exp by the same rule.
+ * The _auto form is two launches, the amax pass and one quantize-transpose, and captures into one graph.
+ * Arguments: the rules, order and codes of the 1-D call with this n, plus: dCt non-NULL when n > 0
+ * (B200VA_ERR_INVALID); rows * cols must not overflow and is at most 2^40 (B200VA_ERR_INVALID); A, C, Ct, d_amax and
+ * d_scale_exp must not meet one another (B200VA_ERR_OVERLAP).  A rejected call writes nothing; rows == 0 or
+ * cols == 0 writes nothing and launches nothing.
+ * Fast path: rows % 16 == 0, cols % 16 == 0 and A, C and Ct on 16-byte boundaries -- every operand torch._scaled_mm
+ * accepts.  Any other shape or placement gives the same bytes through a per-element path that is not tuned.
+ * Asynchronous on `stream`: no allocation, synchronisation or memset; capturable in a CUDA graph. */
+int b200va_quantize_fp8_transpose(int src_dtype, const void *dA, int fp8, void *dC, void *dCt,
+                                  size_t rows, size_t cols, int scale_exp, double *d_amax, void *stream);
+int b200va_quantize_fp8_transpose_auto(int src_dtype, const void *dA, int fp8, void *dC, void *dCt,
+                                       size_t rows, size_t cols, int margin, double *d_amax,
+                                       int32_t *d_scale_exp, void *stream);
 
 /* ---- block-scaled FP8 (MXFP8) quantize and dequantize (row f4) --------------------------------
  * The same two FP8 formats with one scale per block of `block` elements, block one of 32 (OCP Microscaling MXFP8),

@@ -117,6 +117,8 @@ _SIGS = {
     "b200va_dequantize_fp8": (_I, [_I, _P, _I, _P, _SZ, _I, _P]),
     "b200va_quantize_fp8_auto": (_I, [_I, _P, _I, _P, _SZ, _I, _P, _P, _P]),
     "b200va_dequantize_fp8_auto": (_I, [_I, _P, _I, _P, _SZ, _P, _P]),
+    "b200va_quantize_fp8_transpose": (_I, [_I, _P, _I, _P, _P, _SZ, _SZ, _I, _P, _P]),
+    "b200va_quantize_fp8_transpose_auto": (_I, [_I, _P, _I, _P, _P, _SZ, _SZ, _I, _P, _P, _P]),
     "b200va_quantize_mxfp8": (_I, [_I, _P, _I, _P, _P, _SZ, _I, _I, _P]),
     "b200va_dequantize_mxfp8": (_I, [_I, _P, _P, _I, _P, _SZ, _I, _P]),
     "b200va_mxfp8_scale_bytes": (_SZ, [_SZ, _I]),

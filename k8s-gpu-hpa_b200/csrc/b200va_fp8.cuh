@@ -220,19 +220,100 @@ __device__ __forceinline__ void amax_body(const unsigned char* a, size_t n, size
     });
 }
 
+// ---- quantize-transpose ---------------------------------------------------------------------------------
+// b200va_quantize_fp8_transpose: A is rows x cols (row-major, n = rows cols), C gets quant_body's bytes and Ct
+// (cols x rows, row-major) their transpose, Ct[j rows + i] = C[i cols + j], in one pass over A.
+//
+// Tiled path (rows and cols multiples of 16, A, C and Ct on 16-byte boundaries): tiles of T8 x T8 elements, row-major
+// over the matrix and grid-strided, FP8T_THREADS = (T8 / 16) T8 threads per CTA.  Thread t first takes group t % 4
+// of tile row t / 4: it rounds those 16 elements with quant_group, stores the 16 bytes to C, and stores each byte
+// into the shared-memory tile, which holds the tile transposed (tile row j is Ct's row, tile column i is A's row).
+// After the barrier it takes tile row j = t / 4, columns 16 (t % 4) .. + 15: one 16-byte shared load and one 16-byte
+// store to Ct.  So 4 lanes cover the 64 bytes of a Ct row (two whole 32-byte sectors) and a warp 8 Ct rows.  The
+// tile is swizzled: 16-byte chunk h of tile row j sits at chunk h ^ (j / 16), so the byte stores of the 4 lanes of a
+// group (16 tile rows apart) fall in 4 different banks, and a quarter warp's 16-byte loads cover 128 contiguous
+// bytes.  Tiles on the right and bottom edges are partial in steps of 16.  Two tile buffers alternate, so one
+// barrier per tile keeps a tile's reads apart from the writes two tiles later.
+//
+// Element path (every other shape or placement): cast_edges with head = n; element e to C[e] and to
+// Ct[(e % cols) rows + e / cols].  For correctness, not speed.
+constexpr int FP8T_TILE = 64;                                         // T8
+constexpr int FP8T_THREADS = FP8T_TILE / 16 * FP8T_TILE;              // 256
+constexpr int FP8T_SMEM = 2 * FP8T_TILE * FP8T_TILE;                  // two tile buffers, 8 KiB (dynamic)
+
+// The tiled path's body after the dependency wait, one format, n = rows cols elements, k the scale exponent.
+template <int SRC, int F8>
+__device__ __forceinline__ void quant_t_tiles(const unsigned char* a, unsigned char* c, unsigned char* ct, size_t rows,
+                                              size_t cols, int k, amax_bits_t<SRC>& m)
+{
+    constexpr int ES = dt_traits<SRC>::size, T8 = FP8T_TILE;
+    extern __shared__ __align__(16) unsigned char fp8t_tile[];
+    // at most 2^36 / T8 tile columns and 2^40 / (16 T8) tiles (n <= 2^40, rows and cols multiples of 16)
+    const unsigned tiles_c = static_cast<unsigned>((cols + T8 - 1) / T8);
+    const unsigned ntiles = static_cast<unsigned>((rows + T8 - 1) / T8) * tiles_c;
+    const unsigned r = threadIdx.x / 4, q = threadIdx.x % 4;          // phase 1: tile row, group; phase 2: column, rows
+    unsigned buf = 0;
+    for (unsigned t = blockIdx.x; t < ntiles; t += gridDim.x, buf ^= T8 * T8) {
+        const size_t i0 = static_cast<size_t>(t / tiles_c) * T8, j0 = static_cast<size_t>(t % tiles_c) * T8;
+        const unsigned tr = static_cast<unsigned>(min(rows - i0, size_t{T8})), tc = static_cast<unsigned>(min(cols - j0, size_t{T8}));
+        unsigned char* tile = fp8t_tile + buf;
+        if (r < tr && 16 * q < tc) {
+            const size_t e = (i0 + r) * cols + j0 + 16 * q;
+            uint32_t s[4 * ES], d[4];
+            unpack<ES>(ld_vecs<ES>(a + e * ES, 0).v, s);
+            quant_group<SRC, F8>(s, k, m, d);
+            stg128_bits<ST_NA>(c + e, u32x4{d[0], d[1], d[2], d[3]});
+            // byte b goes to tile column 16 q + b, at row r of its swizzled chunk
+            unsigned char* col = tile + 16 * q * T8 + 16 * ((r / 16) ^ q) + r % 16;
+#pragma unroll
+            for (int b = 0; b < 16; ++b) col[b * T8] = static_cast<unsigned char>(d[b / 4] >> (8 * (b % 4)));
+        }
+        __syncthreads();
+        if (r < tc && 16 * q < tr)
+            stg128_bits<ST_NA>(ct + (j0 + r) * rows + i0 + 16 * q,
+                               *reinterpret_cast<const u32x4*>(tile + r * T8 + 16 * (q ^ (r / 16))));
+    }
+}
+
+// The transposed body after the dependency wait: the tiled path for ngroups = n / 16 (head = 0), else the element
+// path (head = n, ngroups = 0).
+template <int SRC, int F8>
+__device__ __forceinline__ void quant_t_body(const unsigned char* a, unsigned char* c, unsigned char* ct, size_t n,
+                                             size_t cols, size_t head, size_t ngroups, int k, amax_bits_t<SRC>& m)
+{
+    constexpr int ES = dt_traits<SRC>::size;
+    const size_t rows = n / cols;
+    if (ngroups) quant_t_tiles<SRC, F8>(a, c, ct, rows, cols, k, m);
+    // e = i cols + j without a 64-bit division, whose call would raise the kernel's register count: e < 2^40, so
+    // e / cols in f64 (by the rounded reciprocal) is within 2^-11 of the quotient, and i is its truncation corrected
+    // by at most one.
+    const double rc = __drcp_rn(static_cast<double>(cols));
+    cast_edges(n, head, head + ngroups * 16, [&](size_t e) {
+        const unsigned char b = quant_elem<SRC, F8>(a + e * ES, k, m);
+        c[e] = b;
+        long long i = static_cast<long long>(static_cast<double>(e) * rc);
+        long long j = static_cast<long long>(e) - i * static_cast<long long>(cols);
+        if (j < 0) { --i; j += cols; }
+        else if (j >= static_cast<long long>(cols)) { ++i; j -= cols; }
+        ct[j * rows + i] = b;
+    });
+}
+
 // One kernel per source type, the format picking one of its two bodies (with_f8).  unroll (1 or 2) and prefetch_first
 // are the launch's geometry, as in convert_vec.  With amax, each CTA max-accumulates its largest |a_i| (as f64 bits)
-// into *amax with one atomic, after the dependency wait like every other access; both bodies reach that one atomic.
+// into *amax with one atomic, after the dependency wait like every other access; every body reaches that one atomic.
 // Without C the kernel is b200va_quantize_fp8_auto's amax pass (amax_body: finite magnitudes only, fmt and k unused).
 // With amax_in, k is auto_scale_exp(*amax_in, fmt, margin) instead of the argument, and thread 0 of CTA 0 writes it
-// to *k_out.
+// to *k_out.  With Ct the kernel is b200va_quantize_fp8_transpose's (quant_t_body; A has `cols` columns, and the
+// launch gives FP8T_THREADS threads and FP8T_SMEM bytes of dynamic shared memory on the tiled path).
 template <int SRC>
 __global__ void fp8_quant_vec(const void* A, void* C, size_t n, size_t head, size_t ngroups, int unroll,
                               int prefetch_first, int fmt, int k, double* amax, const double* amax_in, int margin,
-                              int32_t* k_out)
+                              int32_t* k_out, void* Ct, size_t cols)
 {
     const unsigned char* a = static_cast<const unsigned char*>(A);
     unsigned char* c = static_cast<unsigned char*>(C);
+    unsigned char* ct = static_cast<unsigned char*>(Ct);
     prefetch_first_tile<16, dt_traits<SRC>::size>(prefetch_first, a, head, ngroups, unroll);
     pdl_wait();
 
@@ -244,7 +325,8 @@ __global__ void fp8_quant_vec(const void* A, void* C, size_t n, size_t head, siz
             k = auto_scale_exp(*amax_in, fmt, margin);
             if (blockIdx.x == 0 && threadIdx.x == 0) *k_out = k;
         }
-        with_f8(fmt, [&](auto F8) { quant_body<SRC, F8>(a, c, n, head, ngroups, unroll, k, m); });
+        if (ct) with_f8(fmt, [&](auto F8) { quant_t_body<SRC, F8>(a, c, ct, n, cols, head, ngroups, k, m); });
+        else with_f8(fmt, [&](auto F8) { quant_body<SRC, F8>(a, c, n, head, ngroups, unroll, k, m); });
     }
     if (amax) cta_amax<SRC>(amax, m);
 }

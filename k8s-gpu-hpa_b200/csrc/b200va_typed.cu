@@ -178,7 +178,7 @@ int launch_fp8_typed(const void* dA, void* dC, size_t n, int fmt, int k, double*
                                   QUANT ? 1 : ES, n, QUANT ? 1 : ES);
     if constexpr (QUANT)
         return launch_kernel(fp8_quant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
-                             p.unroll, p.prefetch_first, fmt, k, amax, amax_in, margin, scale_exp);
+                             p.unroll, p.prefetch_first, fmt, k, amax, amax_in, margin, scale_exp, nullptr, size_t{0});
     else
         return launch_kernel(fp8_dequant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
                              p.unroll, p.prefetch_first, fmt, k, static_cast<const int32_t*>(scale_exp));
@@ -196,7 +196,38 @@ int launch_fp8_amax(const void* dA, size_t n, double* amax, cudaStream_t st)
     p.ngroups = (n - p.head) / 16;
     plan_geometry(p, hbm_class(n, ES), p.ngroups, n - p.ngroups * 16);
     return launch_kernel(fp8_quant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, nullptr, n, p.head, p.ngroups,
-                         p.unroll, p.prefetch_first, 0, 0, amax, nullptr, 0, nullptr);
+                         p.unroll, p.prefetch_first, 0, 0, amax, nullptr, 0, nullptr, nullptr, size_t{0});
+}
+
+// b200va_quantize_fp8_transpose (and the quantize pass of its _auto form): one fp8_quant_vec<T> launch with Ct, n =
+// rows cols > 0.  The tiled path runs when rows and cols are multiples of 16 and A, C and Ct sit on 16-byte
+// boundaries: head 0, every group in the body, FP8T_THREADS threads per CTA (one per group of a tile), one tile per
+// CTA and FP8T_SMEM bytes of dynamic shared memory.  Otherwise the element path: head = n, every element an edge
+// item, plan_geometry's threads and grid for A's HBM class.  Neither geometry was tuned.
+template <int T>
+int launch_fp8_transpose(const void* dA, void* dC, void* dCt, size_t rows, size_t cols, int fmt, int k, double* amax,
+                         cudaStream_t st, const double* amax_in = nullptr, int margin = 0, int32_t* scale_exp = nullptr)
+{
+    constexpr size_t ES = dt_traits<T>::size, T8 = FP8T_TILE;
+    const size_t n = rows * cols;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC),
+                    ct = reinterpret_cast<uintptr_t>(dCt);
+    const bool tiled = rows % 16 == 0 && cols % 16 == 0 && ((a | c | ct) & 15u) == 0;
+    cast_plan p{};
+    size_t smem = 0;
+    if (tiled) {
+        const size_t ntiles = (rows + T8 - 1) / T8 * ((cols + T8 - 1) / T8);
+        p.ngroups = n / 16;
+        p.threads = FP8T_THREADS;
+        p.unroll = 1;
+        p.grid = static_cast<unsigned>(std::min<size_t>(ntiles, 0x7fffffff));
+        smem = FP8T_SMEM;
+    } else {
+        p.head = n;
+        plan_geometry(p, hbm_class(n, ES), 0, n);
+    }
+    return launch_kernel(fp8_quant_vec<T>, p.grid, p.threads, smem, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
+                         p.unroll, 0, fmt, k, amax, amax_in, margin, scale_exp, dCt, cols);
 }
 
 // The argument rules the two FP8 entry points share, after the dtype and format codes: scale_exp in [-126, 126],
@@ -220,6 +251,28 @@ int check_scale_exp_arg(size_t es, const void* dA, size_t esc, const void* dC, s
     if (reinterpret_cast<uintptr_t>(d_scale_exp) & 3u) return B200VA_ERR_ALIGN;
     if (ranges_meet(d_scale_exp, 4, dA, n * es) || ranges_meet(d_scale_exp, 4, dC, n * esc) ||
         ranges_meet(d_scale_exp, 4, d_amax, d_amax ? 8 : 0))
+        return B200VA_ERR_OVERLAP;
+    return B200VA_OK;
+}
+
+// The element count of a rows x cols quantize-transpose, saturated at 2^40 + 1 when rows cols overflows, so that the
+// 1-D checks reject it as n > 2^40.
+size_t transpose_n(size_t rows, size_t cols)
+{
+    constexpr size_t past = (size_t{1} << 40) + 1;
+    return cols && rows > past / cols ? past : rows * cols;
+}
+
+// What the two quantize-transpose entry points check after the 1-D calls' checks (check_fp8_args, and
+// check_scale_exp_arg for _auto): dCt non-NULL when n > 0, and its n bytes meeting neither A, C, d_amax nor
+// d_scale_exp (either may be NULL).
+int check_transpose_arg(size_t es, const void* dA, const void* dC, const void* dCt, size_t n, const double* d_amax,
+                        const int32_t* d_scale_exp)
+{
+    if (n == 0) return B200VA_OK;
+    if (!dCt) return B200VA_ERR_INVALID;
+    if (ranges_meet(dCt, n, dA, n * es) || ranges_meet(dCt, n, dC, n) || ranges_meet(dCt, n, d_amax, d_amax ? 8 : 0) ||
+        ranges_meet(dCt, n, d_scale_exp, d_scale_exp ? 4 : 0))
         return B200VA_ERR_OVERLAP;
     return B200VA_OK;
 }
@@ -368,6 +421,43 @@ int b200va_dequantize_fp8_auto(int fp8, const void* dA, int dst_dtype, void* dC,
     with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dst_dtype, [&](auto DST) {
         rc = launch_fp8_typed<false, DST>(dA, dC, n, fp8, 0, nullptr, static_cast<cudaStream_t>(stream), nullptr, 0,
                                           const_cast<int32_t*>(d_scale_exp));
+    });
+    return rc;
+}
+
+int b200va_quantize_fp8_transpose(int src_dtype, const void* dA, int fp8, void* dC, void* dCt, size_t rows, size_t cols,
+                                  int scale_exp, double* d_amax, void* stream)
+{
+    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    const size_t es = dtype_size(src_dtype), n = transpose_n(rows, cols);
+    RC_TRY(check_fp8_args(es, dA, 1, dC, n, scale_exp, d_amax));
+    RC_TRY(check_transpose_arg(es, dA, dC, dCt, n, d_amax, nullptr));
+    if (n == 0) return B200VA_OK;
+    int rc = B200VA_ERR_VARIANT;
+    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(src_dtype, [&](auto SRC) {
+        rc = launch_fp8_transpose<SRC>(dA, dC, dCt, rows, cols, fp8, scale_exp, d_amax, static_cast<cudaStream_t>(stream));
+    });
+    return rc;
+}
+
+int b200va_quantize_fp8_transpose_auto(int src_dtype, const void* dA, int fp8, void* dC, void* dCt, size_t rows,
+                                       size_t cols, int margin, double* d_amax, int32_t* d_scale_exp, void* stream)
+{
+    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    if (margin < 0 || margin > 126 || !d_amax || !d_scale_exp) return B200VA_ERR_INVALID;
+    const size_t es = dtype_size(src_dtype), n = transpose_n(rows, cols);
+    RC_TRY(check_fp8_args(es, dA, 1, dC, n, 0, d_amax));
+    RC_TRY(check_scale_exp_arg(es, dA, 1, dC, n, d_amax, d_scale_exp));
+    RC_TRY(check_transpose_arg(es, dA, dC, dCt, n, d_amax, d_scale_exp));
+    if (n == 0) return B200VA_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int rc = B200VA_ERR_VARIANT;
+    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(src_dtype, [&](auto SRC) {
+        rc = launch_fp8_amax<SRC>(dA, n, d_amax, st);
+        if (rc == B200VA_OK)
+            rc = launch_fp8_transpose<SRC>(dA, dC, dCt, rows, cols, fp8, 0, nullptr, st, d_amax, margin, d_scale_exp);
     });
     return rc;
 }

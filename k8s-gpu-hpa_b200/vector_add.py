@@ -286,6 +286,77 @@ def dequantize_fp8_auto(q, scale_exp, dtype, *, out=None, stream=None):
     return out
 
 
+def _matrix(a) -> tuple[int, int, int]:
+    """(ABI code, rows, cols) of a contiguous 2-D CUDA tensor of f32/f64/f16/bf16."""
+    code = _operand(a, "a")
+    if a.dim() != 2:
+        raise TypeError(f"a must be a 2-D tensor, got {a.dim()} dimensions")
+    return code, a.shape[0], a.shape[1]
+
+
+def _out_shaped(out, dtype, shape, a, name: str):
+    """``out`` checked to be a contiguous tensor of ``dtype`` and ``shape`` on a's device, or a new one."""
+    torch = _torch()
+    if out is None:
+        return torch.empty(shape, dtype=dtype, device=a.device)
+    if (not isinstance(out, torch.Tensor) or out.dtype != dtype or tuple(out.shape) != tuple(shape)
+            or out.device != a.device or not out.is_contiguous()):
+        raise TypeError(f"{name} must be a contiguous {dtype} tensor of shape {list(shape)} on a's device")
+    return out
+
+
+def quantize_fp8_transpose(a, fmt, *, scale_exp: int = 0, amax=None, out=None, out_t=None, stream=None):
+    """The 2-D ``a`` (rows x cols, contiguous, f32/f64/f16/bf16) quantized to FP8 as quantize_fp8 does, and the
+    transpose of the result, in one pass over a (b200va_quantize_fp8_transpose).  ``out`` ([rows, cols]) gets the bytes
+    quantize_fp8 writes for a, ``out_t`` ([cols, rows]) their transpose, both contiguous in the FP8 dtype on a's device
+    (new ones when None).  ``amax``: as in quantize_fp8.  Returns (out, out_t).  rows and cols multiples of 16 with
+    16-byte aligned operands take the tiled path; any other shape gives the same bytes, slowly.
+
+    On an H100 an FP8 GEMM takes both operands K-major, so the backward products of a linear layer use out_t as is:
+    the weight gradient dW = dY^T X is ``torch._scaled_mm(dy_t, x_t.t(), scale_a, scale_b)`` with
+    ``dy_t = quantize_fp8_transpose(dy, ...)[1]`` and ``x_t = quantize_fp8_transpose(x, ...)[1]``: x_t.t() is the
+    column-major mat2 it requires, with no copy.  Asynchronous on the current stream."""
+    torch = _torch()
+    src, rows, cols = _matrix(a)
+    dtype, code = _fp8_format(fmt)
+    out = _out_shaped(out, dtype, (rows, cols), a, "out")
+    out_t = _out_shaped(out_t, dtype, (cols, rows), a, "out_t")
+    if amax is not None:
+        _one_element(amax, torch.float64, a, "amax")
+    with torch.cuda.device(a.device):
+        check(lib.b200va_quantize_fp8_transpose(src, a.data_ptr(), code, out.data_ptr(), out_t.data_ptr(), rows, cols,
+                                                int(scale_exp), amax.data_ptr() if amax is not None else None,
+                                                _stream_ptr(stream)), "b200va_quantize_fp8_transpose")
+    return out, out_t
+
+
+def quantize_fp8_transpose_auto(a, fmt, *, margin: int = 0, amax=None, scale_exp=None, out=None, out_t=None,
+                                stream=None):
+    """quantize_fp8_auto of the 2-D ``a`` with the transpose of the result (b200va_quantize_fp8_transpose_auto): the
+    amax pass, then one quantize-transpose with the k chosen on the device.  ``amax``, ``scale_exp`` and ``margin`` as
+    in quantize_fp8_auto, ``out`` and ``out_t`` as in quantize_fp8_transpose.  Returns (out, out_t, scale_exp) without
+    a host sync; torch.exp2(-scale_exp.float()) is the scale torch._scaled_mm takes for out or out_t.t().
+    Asynchronous on the current stream."""
+    torch = _torch()
+    src, rows, cols = _matrix(a)
+    dtype, code = _fp8_format(fmt)
+    out = _out_shaped(out, dtype, (rows, cols), a, "out")
+    out_t = _out_shaped(out_t, dtype, (cols, rows), a, "out_t")
+    if amax is not None:
+        _one_element(amax, torch.float64, a, "amax")
+    scale_exp = (torch.empty(1, dtype=torch.int32, device=a.device) if scale_exp is None
+                 else _one_element(scale_exp, torch.int32, a, "scale_exp"))
+    with torch.cuda.device(a.device):
+        st = stream if stream is not None else torch.cuda.current_stream()
+        if amax is None:
+            with torch.cuda.stream(st):
+                amax = torch.zeros(1, dtype=torch.float64, device=a.device)
+        check(lib.b200va_quantize_fp8_transpose_auto(src, a.data_ptr(), code, out.data_ptr(), out_t.data_ptr(), rows,
+                                                     cols, int(margin), amax.data_ptr(), scale_exp.data_ptr(),
+                                                     st.cuda_stream), "b200va_quantize_fp8_transpose_auto")
+    return out, out_t, scale_exp
+
+
 _U64 = (1 << 64) - 1
 
 

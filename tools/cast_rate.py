@@ -1,6 +1,6 @@
 """Rate of the cast kernels by family, next to the f32 COPY and READ2 ceiling probes, in one process.
 
-    python tools/cast_rate.py [--family convert|fp8|mxfp8|sr|all] [--log2n 28] [--calls 20] [--rounds 3]
+    python tools/cast_rate.py [--family convert|fp8|fp8t|mxfp8|sr|all] [--log2n 28] [--calls 20] [--rounds 3]
 
 Per round, every op of the chosen families is timed at n elements with CUDA events around `calls` back-to-back calls
 (after two warm-up calls), then b200va_probe_f32 COPY (8 n bytes) and READ2 (8 n read) at the same n.  The families
@@ -14,6 +14,11 @@ and the algorithmic bytes of one call:
            k chosen on the device, n * (2 sizeof T + 1).  "us" is the time of the whole recipe, "TB/s" counts what
            it moves; neither resets the amax between calls (a running max).  Last, b200va_dequantize_fp8_auto with
            the device k, n * (sizeof T + 1).
+  fp8t     the quantize-transpose at 8192 x 8192, 16384 x 16384, 4096 x 32768 and 32768 x 4096 (not at n) from each
+           type to E4M3, and to E5M2 at 8192 x 8192, next to: b200va_quantize_fp8 alone (the floor: read A, write
+           C), the same followed by torch's transpose of the FP8 result into a preallocated tensor, the _auto form,
+           and b200va_quantize_fp8_auto followed by torch's transpose.  Every entry counts n * (sizeof T + 2) bytes,
+           what the fused call moves, so the rates compare times.
   mxfp8    per type and format, alternated in this order: quantize and dequantize at block 32 and at block 128,
            n * (sizeof T + 1 + 1 / block); the per-tensor recipes they compete with are in the fp8 family.
   sr       the stochastically rounding casts from f32, each beside its round-to-nearest counterpart: to f16 and bf16,
@@ -98,6 +103,41 @@ def fp8_ops(torch, va, n, tdt, f8):
         del a, amax
 
 
+FP8T_SHAPES = ((8192, 8192), (16384, 16384), (4096, 32768), (32768, 4096))
+
+
+def fp8t_ops(torch, va, n, tdt, f8):
+    """n is unused: the quantize-transpose family runs at FP8T_SHAPES."""
+    for rows, cols in FP8T_SHAPES:
+        m = rows * cols
+        for s in tdt:
+            a = torch.randn(rows, cols, dtype=torch.float32, device="cuda").to(tdt[s])
+            amax = torch.zeros(1, dtype=torch.float64, device="cuda")
+            k = torch.zeros(1, dtype=torch.int32, device="cuda")
+            nbytes = m * (SIZE[s] + 2)
+            for f in (("e4m3", "e5m2") if (rows, cols) == (8192, 8192) else ("e4m3",)):
+                q = torch.empty(rows, cols, dtype=f8[f], device="cuda")
+                qt = torch.empty(cols, rows, dtype=f8[f], device="cuda")
+                tag = f"{s}->{f} {rows}x{cols}"
+
+                def recipe1():
+                    va.quantize_fp8(a, f8[f], out=q)
+                    qt.copy_(q.t())
+
+                def recipe1_auto():
+                    va.quantize_fp8_auto(a, f8[f], amax=amax, scale_exp=k, out=q)
+                    qt.copy_(q.t())
+
+                yield f"quantize_fp8_transpose {tag}", lambda: va.quantize_fp8_transpose(a, f8[f], out=q, out_t=qt), nbytes
+                yield f"quantize_fp8 alone {tag}", lambda: va.quantize_fp8(a, f8[f], out=q), nbytes
+                yield f"quantize_fp8 + torch transpose {tag}", recipe1, nbytes
+                yield (f"quantize_fp8_transpose_auto {tag}",
+                       lambda: va.quantize_fp8_transpose_auto(a, f8[f], amax=amax, scale_exp=k, out=q, out_t=qt), nbytes)
+                yield f"quantize_fp8_auto + torch transpose {tag}", recipe1_auto, nbytes
+                del q, qt
+            del a, amax, k
+
+
 def mxfp8_ops(torch, va, n, tdt, f8):
     for s in tdt:
         a = torch.randn(n, dtype=torch.float32, device="cuda").to(tdt[s])
@@ -143,7 +183,7 @@ def sr_ops(torch, va, n, tdt, f8):
     del a, amax, c
 
 
-FAMILIES = {"convert": convert_ops, "fp8": fp8_ops, "mxfp8": mxfp8_ops, "sr": sr_ops}
+FAMILIES = {"convert": convert_ops, "fp8": fp8_ops, "fp8t": fp8t_ops, "mxfp8": mxfp8_ops, "sr": sr_ops}
 
 
 def main() -> None:
