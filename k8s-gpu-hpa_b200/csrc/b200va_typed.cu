@@ -165,116 +165,155 @@ int launch_convert_typed(const void* dA, void* dC, size_t n, cudaStream_t st)
                          p.unroll, p.prefetch_first);
 }
 
-// b200va_quantize_fp8 (QUANT: T -> fmt) and b200va_dequantize_fp8 (fmt -> T): one fp8_quant_vec<T> or
-// fp8_dequant_vec<T> launch, the format passed to the kernel.  A unit is a group of 16 when quantizing and a 16-byte
-// output slice (sizeof T per group) when dequantizing.  The _auto forms pass the device-side k: quantize reads the
-// amax at amax_in and writes k to *scale_exp, dequantize reads k from *scale_exp.
-template <bool QUANT, int T>
-int launch_fp8_typed(const void* dA, void* dC, size_t n, int fmt, int k, double* amax, cudaStream_t st,
-                     const double* amax_in = nullptr, int margin = 0, int32_t* scale_exp = nullptr)
+// The arguments of one fp8_quant_vec launch besides its plan, set by name; a launch that sets only a, c, n, fmt, k and
+// amax is the 1-D quantize by the host's k.  The kernel's mode follows from which pointers are set (b200va_fp8.cuh):
+//   amax pass   c NULL: max-accumulates A's largest finite |a_i| into *amax and stores nothing (fmt and k unused)
+//   auto k      amax_in: k = auto_scale_exp(*amax_in, fmt, margin), written to *k_out
+//   transpose   ct: C's transpose also goes to Ct, A having `cols` columns
+struct fp8_quant_args {
+    const void* a = nullptr;
+    void* c = nullptr;
+    size_t n = 0;
+    int fmt = 0, k = 0;
+    double* amax = nullptr;
+    const double* amax_in = nullptr;
+    int margin = 0;
+    int32_t* k_out = nullptr;
+    void* ct = nullptr;
+    size_t cols = 0;
+};
+
+using fp8_quant_fn = decltype(&fp8_quant_vec<DT_F32>);
+
+// The one launch site of fp8_quant_vec: fn = fp8_quant_vec<T> under plan p, with smem bytes of dynamic shared memory.
+int launch_fp8_quant(fp8_quant_fn fn, const cast_plan& p, size_t smem, const fp8_quant_args& q, cudaStream_t st)
 {
-    constexpr size_t ES = dt_traits<T>::size;
-    const cast_plan p = plan_cast(reinterpret_cast<uintptr_t>(dA), QUANT ? ES : 1, reinterpret_cast<uintptr_t>(dC),
-                                  QUANT ? 1 : ES, n, QUANT ? 1 : ES);
-    if constexpr (QUANT)
-        return launch_kernel(fp8_quant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
-                             p.unroll, p.prefetch_first, fmt, k, amax, amax_in, margin, scale_exp, nullptr, size_t{0});
-    else
-        return launch_kernel(fp8_dequant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
-                             p.unroll, p.prefetch_first, fmt, k, static_cast<const int32_t*>(scale_exp));
+    return launch_kernel(fn, p.grid, p.threads, smem, st, pdl_enabled(), q.a, q.c, q.n, p.head, p.ngroups, p.unroll,
+                         p.prefetch_first, q.fmt, q.k, q.amax, q.amax_in, q.margin, q.k_out, q.ct, q.cols);
 }
 
-// b200va_quantize_fp8_auto's amax pass: one fp8_quant_vec<T> launch without C.  There is no C to share a phase with,
-// so the vector body starts at the head that puts A alone on a 16-byte boundary; a unit is a group of 16, and every
-// element outside the body an edge item.  The geometry follows A's HBM class.
-template <int T>
-int launch_fp8_amax(const void* dA, size_t n, double* amax, cudaStream_t st)
+// The amax pass's plan, over n elements of es bytes at a.  There is no C to share a phase with, so the vector body
+// starts at the head that puts A alone on a 16-byte boundary; a unit is a group of 16, and every element outside the
+// body an edge item.  The geometry follows A's HBM class.
+cast_plan plan_fp8_amax(uintptr_t a, size_t es, size_t n)
 {
-    constexpr size_t ES = dt_traits<T>::size;
     cast_plan p{};
-    p.head = std::min(head_peel(reinterpret_cast<uintptr_t>(dA), ES), n);
+    p.head = std::min(head_peel(a, es), n);
     p.ngroups = (n - p.head) / 16;
-    plan_geometry(p, hbm_class(n, ES), p.ngroups, n - p.ngroups * 16);
-    return launch_kernel(fp8_quant_vec<T>, p.grid, p.threads, 0, st, pdl_enabled(), dA, nullptr, n, p.head, p.ngroups,
-                         p.unroll, p.prefetch_first, 0, 0, amax, nullptr, 0, nullptr, nullptr, size_t{0});
+    plan_geometry(p, hbm_class(n, es), p.ngroups, n - p.ngroups * 16);
+    return p;
 }
 
-// b200va_quantize_fp8_transpose (and the quantize pass of its _auto form): one fp8_quant_vec<T> launch with Ct, n =
-// rows cols > 0.  The tiled path runs when rows and cols are multiples of 16 and A, C and Ct sit on 16-byte
-// boundaries: head 0, every group in the body, FP8T_THREADS threads per CTA (one per group of a tile), one tile per
-// CTA and FP8T_SMEM bytes of dynamic shared memory.  Otherwise the element path: head = n, every element an edge
-// item, plan_geometry's threads and grid for A's HBM class.  Neither geometry was tuned.
-template <int T>
-int launch_fp8_transpose(const void* dA, void* dC, void* dCt, size_t rows, size_t cols, int fmt, int k, double* amax,
-                         cudaStream_t st, const double* amax_in = nullptr, int margin = 0, int32_t* scale_exp = nullptr)
+// The quantize-transpose's plan, n = rows cols > 0 elements of es bytes.  The tiled path runs when rows and cols are
+// multiples of 16 and A, C and Ct sit on 16-byte boundaries: head 0, every group in the body, FP8T_THREADS threads per
+// CTA (one per group of a tile), one tile per CTA and FP8T_SMEM bytes of dynamic shared memory (smem).  Otherwise the
+// element path: head = n, every element an edge item, plan_geometry's threads and grid for A's HBM class.  Neither
+// path prefetches a first tile, and neither geometry was tuned.
+cast_plan plan_fp8_transpose(uintptr_t a, uintptr_t c, uintptr_t ct, size_t es, size_t rows, size_t cols, size_t& smem)
 {
-    constexpr size_t ES = dt_traits<T>::size, T8 = FP8T_TILE;
+    constexpr size_t T8 = FP8T_TILE;
     const size_t n = rows * cols;
-    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC),
-                    ct = reinterpret_cast<uintptr_t>(dCt);
-    const bool tiled = rows % 16 == 0 && cols % 16 == 0 && ((a | c | ct) & 15u) == 0;
     cast_plan p{};
-    size_t smem = 0;
-    if (tiled) {
-        const size_t ntiles = (rows + T8 - 1) / T8 * ((cols + T8 - 1) / T8);
+    smem = 0;
+    if (rows % 16 == 0 && cols % 16 == 0 && ((a | c | ct) & 15u) == 0) {
         p.ngroups = n / 16;
         p.threads = FP8T_THREADS;
         p.unroll = 1;
-        p.grid = static_cast<unsigned>(std::min<size_t>(ntiles, 0x7fffffff));
+        p.grid = static_cast<unsigned>(std::min<size_t>((rows + T8 - 1) / T8 * ((cols + T8 - 1) / T8), 0x7fffffff));
         smem = FP8T_SMEM;
     } else {
         p.head = n;
-        plan_geometry(p, hbm_class(n, ES), 0, n);
+        plan_geometry(p, hbm_class(n, es), 0, n);
+        p.prefetch_first = 0;
     }
-    return launch_kernel(fp8_quant_vec<T>, p.grid, p.threads, smem, st, pdl_enabled(), dA, dC, n, p.head, p.ngroups,
-                         p.unroll, 0, fmt, k, amax, amax_in, margin, scale_exp, dCt, cols);
+    return p;
 }
 
-// The argument rules the two FP8 entry points share, after the dtype and format codes: scale_exp in [-126, 126],
-// then A and C as b200va_convert checks them (1-byte FP8 elements), then d_amax (may be NULL) 8-byte aligned and
-// meeting neither A nor C.
-int check_fp8_args(size_t es, const void* dA, size_t esc, const void* dC, size_t n, int k, const double* d_amax)
+// The argument rules of every per-tensor FP8 cast after the dtype and format codes, in the order they apply.  A holds
+// n elements of esa bytes and C n of esc, one side FP8 (a quantize has esc = 1).
+//   1. k is the host's scale exponent, in [-126, 126]; with auto_k it is the margin, in [0, 126], d_scale_exp is
+//      non-NULL, and a quantize's d_amax is non-NULL.
+//   2. A and C as b200va_convert checks them.
+//   3. d_amax (may be NULL) 8-byte aligned and meeting neither A nor C.
+//   4. d_scale_exp (may be NULL) 4-byte aligned and meeting neither A, C nor d_amax.
+//   5. For a quantize-transpose with n > 0: dCt non-NULL, and its n bytes meeting none of the others.
+int check_fp8_args(size_t esa, const void* dA, size_t esc, const void* dC, size_t n, int k, bool auto_k,
+                   const double* d_amax, const int32_t* d_scale_exp, bool transpose, const void* dCt)
 {
-    if (k < -126 || k > 126) return B200VA_ERR_INVALID;
-    RC_TRY(check_convert_operands(es, dA, esc, dC, n));
+    if (k < (auto_k ? 0 : -126) || k > 126 || (auto_k && (!d_scale_exp || (esc == 1 && !d_amax))))
+        return B200VA_ERR_INVALID;
+    RC_TRY(check_convert_operands(esa, dA, esc, dC, n));
+    const size_t abytes = n * esa, cbytes = n * esc, mbytes = d_amax ? 8 : 0, sbytes = d_scale_exp ? 4 : 0;
     if (reinterpret_cast<uintptr_t>(d_amax) & 7u) return B200VA_ERR_ALIGN;
-    if (d_amax && (ranges_meet(d_amax, 8, dA, n * es) || ranges_meet(d_amax, 8, dC, n * esc)))
-        return B200VA_ERR_OVERLAP;
-    return B200VA_OK;
-}
-
-// What the two _auto entry points check after check_fp8_args: d_scale_exp (non-NULL) 4-byte aligned and meeting
-// neither A, C nor d_amax (NULL for dequantize).
-int check_scale_exp_arg(size_t es, const void* dA, size_t esc, const void* dC, size_t n, const double* d_amax,
-                        const int32_t* d_scale_exp)
-{
+    if (ranges_meet(d_amax, mbytes, dA, abytes) || ranges_meet(d_amax, mbytes, dC, cbytes)) return B200VA_ERR_OVERLAP;
     if (reinterpret_cast<uintptr_t>(d_scale_exp) & 3u) return B200VA_ERR_ALIGN;
-    if (ranges_meet(d_scale_exp, 4, dA, n * es) || ranges_meet(d_scale_exp, 4, dC, n * esc) ||
-        ranges_meet(d_scale_exp, 4, d_amax, d_amax ? 8 : 0))
+    if (ranges_meet(d_scale_exp, sbytes, dA, abytes) || ranges_meet(d_scale_exp, sbytes, dC, cbytes) ||
+        ranges_meet(d_scale_exp, sbytes, d_amax, mbytes))
         return B200VA_ERR_OVERLAP;
-    return B200VA_OK;
-}
-
-// The element count of a rows x cols quantize-transpose, saturated at 2^40 + 1 when rows cols overflows, so that the
-// 1-D checks reject it as n > 2^40.
-size_t transpose_n(size_t rows, size_t cols)
-{
-    constexpr size_t past = (size_t{1} << 40) + 1;
-    return cols && rows > past / cols ? past : rows * cols;
-}
-
-// What the two quantize-transpose entry points check after the 1-D calls' checks (check_fp8_args, and
-// check_scale_exp_arg for _auto): dCt non-NULL when n > 0, and its n bytes meeting neither A, C, d_amax nor
-// d_scale_exp (either may be NULL).
-int check_transpose_arg(size_t es, const void* dA, const void* dC, const void* dCt, size_t n, const double* d_amax,
-                        const int32_t* d_scale_exp)
-{
-    if (n == 0) return B200VA_OK;
+    if (!transpose || n == 0) return B200VA_OK;
     if (!dCt) return B200VA_ERR_INVALID;
-    if (ranges_meet(dCt, n, dA, n * es) || ranges_meet(dCt, n, dC, n) || ranges_meet(dCt, n, d_amax, d_amax ? 8 : 0) ||
-        ranges_meet(dCt, n, d_scale_exp, d_scale_exp ? 4 : 0))
+    if (ranges_meet(dCt, n, dA, abytes) || ranges_meet(dCt, n, dC, cbytes) || ranges_meet(dCt, n, d_amax, mbytes) ||
+        ranges_meet(dCt, n, d_scale_exp, sbytes))
         return B200VA_ERR_OVERLAP;
     return B200VA_OK;
+}
+
+// Every per-tensor FP8 quantize.  The shape is n = rows cols elements; with `transpose`, C's transpose also goes to
+// dCt, A having `cols` columns.  The scale is the host's k; with auto_k, k is the margin, and an amax pass into
+// *d_amax comes first, from which the quantize launch chooses the exponent and writes it to *d_scale_exp.
+int quantize_fp8(int src_dtype, const void* dA, int fp8, void* dC, size_t rows, size_t cols, void* dCt, bool transpose,
+                 int k, bool auto_k, double* d_amax, int32_t* d_scale_exp, void* stream)
+{
+    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    // rows cols, saturated at 2^40 + 1 when the product overflows, so that the operand checks reject it as n > 2^40
+    constexpr size_t past = (size_t{1} << 40) + 1;
+    const size_t es = dtype_size(src_dtype), n = cols && rows > past / cols ? past : rows * cols;
+    RC_TRY(check_fp8_args(es, dA, 1, dC, n, k, auto_k, d_amax, d_scale_exp, transpose, dCt));
+    if (n == 0) return B200VA_OK;
+    fp8_quant_fn fn = nullptr;
+    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(src_dtype, [&](auto SRC) { fn = fp8_quant_vec<SRC>; });
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC);
+    fp8_quant_args q;
+    q.a = dA;
+    q.n = n;
+    if (auto_k) {
+        q.amax = d_amax;                                                    // the amax pass: no C yet
+        RC_TRY(launch_fp8_quant(fn, plan_fp8_amax(a, es, n), 0, q, st));
+        q.amax = nullptr;
+        q.amax_in = d_amax;
+        q.margin = k;
+        q.k_out = d_scale_exp;
+    } else {
+        q.k = k;
+        q.amax = d_amax;
+    }
+    q.c = dC;
+    q.fmt = fp8;
+    if (!transpose) return launch_fp8_quant(fn, plan_cast(a, es, c, 1, n, 1), 0, q, st);
+    q.ct = dCt;
+    q.cols = cols;
+    size_t smem = 0;
+    const cast_plan p = plan_fp8_transpose(a, c, reinterpret_cast<uintptr_t>(dCt), es, rows, cols, smem);
+    return launch_fp8_quant(fn, p, smem, q, st);
+}
+
+// Every per-tensor FP8 dequantize: one fp8_dequant_vec<T> launch, a unit being a 16-byte output slice (sizeof T per
+// group of 16).  The scale is the host's k; with auto_k the kernel reads k from *k_in.
+int dequantize_fp8(int fp8, const void* dA, int dst_dtype, void* dC, size_t n, int k, bool auto_k, const int32_t* k_in,
+                   void* stream)
+{
+    if (dst_dtype < 0 || dst_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    const size_t es = dtype_size(dst_dtype);
+    RC_TRY(check_fp8_args(1, dA, es, dC, n, k, auto_k, nullptr, k_in, false, nullptr));
+    if (n == 0) return B200VA_OK;
+    decltype(&fp8_dequant_vec<DT_F32>) fn = nullptr;
+    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dst_dtype, [&](auto DST) { fn = fp8_dequant_vec<DST>; });
+    const cast_plan p = plan_cast(reinterpret_cast<uintptr_t>(dA), 1, reinterpret_cast<uintptr_t>(dC), es, n, es);
+    return launch_kernel(fn, p.grid, p.threads, 0, static_cast<cudaStream_t>(stream), pdl_enabled(), dA, dC, n, p.head,
+                         p.ngroups, p.unroll, p.prefetch_first, fp8, k, k_in);
 }
 
 // b200va_convert_sr_f32 and b200va_quantize_fp8_sr_f32: one sr_cast_vec launch, a group per unit, dst one of SR_*.
@@ -364,102 +403,36 @@ int b200va_convert(int src_dtype, const void* dA, int dst_dtype, void* dC, size_
 int b200va_quantize_fp8(int src_dtype, const void* dA, int fp8, void* dC, size_t n, int scale_exp, double* d_amax,
                         void* stream)
 {
-    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
-    RC_TRY(current_dev_info(nullptr));
-    RC_TRY(check_fp8_args(dtype_size(src_dtype), dA, 1, dC, n, scale_exp, d_amax));
-    if (n == 0) return B200VA_OK;
-    int rc = B200VA_ERR_VARIANT;
-    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(src_dtype, [&](auto SRC) {
-        rc = launch_fp8_typed<true, SRC>(dA, dC, n, fp8, scale_exp, d_amax, static_cast<cudaStream_t>(stream));
-    });
-    return rc;
+    return quantize_fp8(src_dtype, dA, fp8, dC, n, 1, nullptr, false, scale_exp, false, d_amax, nullptr, stream);
 }
 
 int b200va_dequantize_fp8(int fp8, const void* dA, int dst_dtype, void* dC, size_t n, int scale_exp, void* stream)
 {
-    if (dst_dtype < 0 || dst_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
-    RC_TRY(current_dev_info(nullptr));
-    RC_TRY(check_fp8_args(1, dA, dtype_size(dst_dtype), dC, n, scale_exp, nullptr));
-    if (n == 0) return B200VA_OK;
-    int rc = B200VA_ERR_VARIANT;
-    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dst_dtype, [&](auto DST) {
-        rc = launch_fp8_typed<false, DST>(dA, dC, n, fp8, scale_exp, nullptr, static_cast<cudaStream_t>(stream));
-    });
-    return rc;
+    return dequantize_fp8(fp8, dA, dst_dtype, dC, n, scale_exp, false, nullptr, stream);
 }
 
 int b200va_quantize_fp8_auto(int src_dtype, const void* dA, int fp8, void* dC, size_t n, int margin, double* d_amax,
                              int32_t* d_scale_exp, void* stream)
 {
-    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
-    RC_TRY(current_dev_info(nullptr));
-    if (margin < 0 || margin > 126 || !d_amax || !d_scale_exp) return B200VA_ERR_INVALID;
-    const size_t es = dtype_size(src_dtype);
-    RC_TRY(check_fp8_args(es, dA, 1, dC, n, 0, d_amax));
-    RC_TRY(check_scale_exp_arg(es, dA, 1, dC, n, d_amax, d_scale_exp));
-    if (n == 0) return B200VA_OK;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int rc = B200VA_ERR_VARIANT;
-    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(src_dtype, [&](auto SRC) {
-        rc = launch_fp8_amax<SRC>(dA, n, d_amax, st);
-        if (rc == B200VA_OK) rc = launch_fp8_typed<true, SRC>(dA, dC, n, fp8, 0, nullptr, st, d_amax, margin, d_scale_exp);
-    });
-    return rc;
+    return quantize_fp8(src_dtype, dA, fp8, dC, n, 1, nullptr, false, margin, true, d_amax, d_scale_exp, stream);
 }
 
 int b200va_dequantize_fp8_auto(int fp8, const void* dA, int dst_dtype, void* dC, size_t n, const int32_t* d_scale_exp,
                                void* stream)
 {
-    if (dst_dtype < 0 || dst_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
-    RC_TRY(current_dev_info(nullptr));
-    if (!d_scale_exp) return B200VA_ERR_INVALID;
-    const size_t es = dtype_size(dst_dtype);
-    RC_TRY(check_fp8_args(1, dA, es, dC, n, 0, nullptr));
-    RC_TRY(check_scale_exp_arg(1, dA, es, dC, n, nullptr, d_scale_exp));
-    if (n == 0) return B200VA_OK;
-    int rc = B200VA_ERR_VARIANT;
-    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(dst_dtype, [&](auto DST) {
-        rc = launch_fp8_typed<false, DST>(dA, dC, n, fp8, 0, nullptr, static_cast<cudaStream_t>(stream), nullptr, 0,
-                                          const_cast<int32_t*>(d_scale_exp));
-    });
-    return rc;
+    return dequantize_fp8(fp8, dA, dst_dtype, dC, n, 0, true, d_scale_exp, stream);
 }
 
 int b200va_quantize_fp8_transpose(int src_dtype, const void* dA, int fp8, void* dC, void* dCt, size_t rows, size_t cols,
                                   int scale_exp, double* d_amax, void* stream)
 {
-    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
-    RC_TRY(current_dev_info(nullptr));
-    const size_t es = dtype_size(src_dtype), n = transpose_n(rows, cols);
-    RC_TRY(check_fp8_args(es, dA, 1, dC, n, scale_exp, d_amax));
-    RC_TRY(check_transpose_arg(es, dA, dC, dCt, n, d_amax, nullptr));
-    if (n == 0) return B200VA_OK;
-    int rc = B200VA_ERR_VARIANT;
-    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(src_dtype, [&](auto SRC) {
-        rc = launch_fp8_transpose<SRC>(dA, dC, dCt, rows, cols, fp8, scale_exp, d_amax, static_cast<cudaStream_t>(stream));
-    });
-    return rc;
+    return quantize_fp8(src_dtype, dA, fp8, dC, rows, cols, dCt, true, scale_exp, false, d_amax, nullptr, stream);
 }
 
 int b200va_quantize_fp8_transpose_auto(int src_dtype, const void* dA, int fp8, void* dC, void* dCt, size_t rows,
                                        size_t cols, int margin, double* d_amax, int32_t* d_scale_exp, void* stream)
 {
-    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
-    RC_TRY(current_dev_info(nullptr));
-    if (margin < 0 || margin > 126 || !d_amax || !d_scale_exp) return B200VA_ERR_INVALID;
-    const size_t es = dtype_size(src_dtype), n = transpose_n(rows, cols);
-    RC_TRY(check_fp8_args(es, dA, 1, dC, n, 0, d_amax));
-    RC_TRY(check_scale_exp_arg(es, dA, 1, dC, n, d_amax, d_scale_exp));
-    RC_TRY(check_transpose_arg(es, dA, dC, dCt, n, d_amax, d_scale_exp));
-    if (n == 0) return B200VA_OK;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int rc = B200VA_ERR_VARIANT;
-    with_value<DT_F32, DT_F64, DT_F16, DT_BF16>(src_dtype, [&](auto SRC) {
-        rc = launch_fp8_amax<SRC>(dA, n, d_amax, st);
-        if (rc == B200VA_OK)
-            rc = launch_fp8_transpose<SRC>(dA, dC, dCt, rows, cols, fp8, 0, nullptr, st, d_amax, margin, d_scale_exp);
-    });
-    return rc;
+    return quantize_fp8(src_dtype, dA, fp8, dC, rows, cols, dCt, true, margin, true, d_amax, d_scale_exp, stream);
 }
 
 int b200va_convert_sr_f32(const float* dA, int dst_dtype, void* dC, size_t n, uint64_t seed, uint64_t first,
@@ -478,7 +451,7 @@ int b200va_quantize_fp8_sr_f32(const float* dA, int fp8, void* dC, size_t n, int
 {
     if (fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
     RC_TRY(current_dev_info(nullptr));
-    RC_TRY(check_fp8_args(4, dA, 1, dC, n, scale_exp, d_amax));
+    RC_TRY(check_fp8_args(4, dA, 1, dC, n, scale_exp, false, d_amax, nullptr, false, nullptr));
     if (n == 0) return B200VA_OK;
     return launch_sr(dA, fp8 == F8_E4M3 ? SR_E4M3 : SR_E5M2, dC, n, scale_exp, seed, first, d_amax,
                      static_cast<cudaStream_t>(stream));

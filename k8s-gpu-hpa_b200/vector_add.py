@@ -200,41 +200,6 @@ def convert(a, dtype, out=None, *, stream=None):
     return out
 
 
-def quantize_fp8(a, fmt, *, scale_exp: int = 0, amax=None, out=None, stream=None):
-    """``a`` (f32/f64/f16/bf16) times 2^scale_exp, rounded once to FP8 (b200va_quantize_fp8): round-to-nearest-even,
-    saturating at +-max finite (448 for E4M3, 57344 for E5M2), inf included; NaN stays NaN.  ``fmt``:
-    torch.float8_e4m3fn / torch.float8_e5m2 or "e4m3" / "e5m2".  ``amax``: a one-element float64 CUDA tensor that
-    max-accumulates max |a| (unscaled; NaN if any element is); set it to 0 before the first call.  ``out``: a
-    contiguous CUDA tensor of the FP8 dtype with a's length on a's device, else a new one.  Asynchronous on the
-    current stream."""
-    torch = _torch()
-    src = _operand(a, "a")
-    dtype, code = _fp8_format(fmt)
-    out = _out(out, dtype, a)
-    if amax is not None and (not isinstance(amax, torch.Tensor) or amax.dtype != torch.float64 or amax.numel() != 1
-                             or amax.device != a.device):
-        raise TypeError("amax must be a one-element float64 tensor on a's device")
-    with torch.cuda.device(a.device):
-        check(lib.b200va_quantize_fp8(src, a.data_ptr(), code, out.data_ptr(), a.numel(), int(scale_exp),
-                                      amax.data_ptr() if amax is not None else None, _stream_ptr(stream)),
-              "b200va_quantize_fp8")
-    return out
-
-
-def dequantize_fp8(a, dtype, *, scale_exp: int = 0, out=None, stream=None):
-    """FP8 ``a`` (torch.float8_e4m3fn / float8_e5m2) times 2^-scale_exp, rounded once to ``dtype``
-    (torch.float32/float64/float16/bfloat16, or "f32"/"f64"/"f16"/"bf16") by b200va_dequantize_fp8: round-to-nearest-
-    even, no FTZ, overflow to inf.  ``out``: a contiguous CUDA tensor of ``dtype`` with a's length on a's device, else
-    a new one.  Asynchronous on the current stream."""
-    code = _operand(a, "a", _fp8_format)
-    dtype, dst = _float_dtype(dtype)
-    out = _out(out, dtype, a)
-    with _torch().cuda.device(a.device):
-        check(lib.b200va_dequantize_fp8(code, a.data_ptr(), dst, out.data_ptr(), a.numel(), int(scale_exp),
-                                        _stream_ptr(stream)), "b200va_dequantize_fp8")
-    return out
-
-
 def _one_element(t, dtype, a, name: str):
     """``t`` checked to be a one-element tensor of ``dtype`` on a's device."""
     torch = _torch()
@@ -243,47 +208,9 @@ def _one_element(t, dtype, a, name: str):
     return t
 
 
-def quantize_fp8_auto(a, fmt, *, margin: int = 0, amax=None, scale_exp=None, out=None, stream=None):
-    """``a`` (f32/f64/f16/bf16) quantized to FP8 with a power-of-two scale 2^k chosen on the device from the amax
-    (b200va_quantize_fp8_auto): an amax pass max-accumulates the largest finite |a| into ``amax``, then k is the
-    largest exponent with amax 2^k <= max finite (448 for E4M3, 57344 for E5M2), less ``margin`` (0..126), clamped to
-    [-126, 126], and a[i] 2^k is rounded once by quantize_fp8's rules.  With margin >= 0, only +-inf saturates.
-    ``amax``: a one-element float64 CUDA tensor, the caller's running max; None makes a zeroed one on the stream
-    (current scaling).  ``scale_exp``: a one-element int32 CUDA tensor that receives k, else a new one.  ``out``: as
-    in quantize_fp8.  Returns (out, scale_exp) without a host sync; torch.exp2(-scale_exp.float()) is the per-tensor
-    dequantization scale a tensor-wise torch._scaled_mm takes.  Asynchronous on the current stream."""
-    torch = _torch()
-    src = _operand(a, "a")
-    dtype, code = _fp8_format(fmt)
-    out = _out(out, dtype, a)
-    if amax is not None:
-        _one_element(amax, torch.float64, a, "amax")
-    scale_exp = (torch.empty(1, dtype=torch.int32, device=a.device) if scale_exp is None
-                 else _one_element(scale_exp, torch.int32, a, "scale_exp"))
-    with torch.cuda.device(a.device):
-        st = stream if stream is not None else torch.cuda.current_stream()
-        if amax is None:
-            with torch.cuda.stream(st):
-                amax = torch.zeros(1, dtype=torch.float64, device=a.device)
-        check(lib.b200va_quantize_fp8_auto(src, a.data_ptr(), code, out.data_ptr(), a.numel(), int(margin),
-                                           amax.data_ptr(), scale_exp.data_ptr(), st.cuda_stream),
-              "b200va_quantize_fp8_auto")
-    return out, scale_exp
-
-
-def dequantize_fp8_auto(q, scale_exp, dtype, *, out=None, stream=None):
-    """FP8 ``q`` times 2^-k, k the one-element int32 CUDA tensor ``scale_exp`` that quantize_fp8_auto wrote, rounded
-    once to ``dtype`` by dequantize_fp8's rules (b200va_dequantize_fp8_auto); k is read on the device, and one outside
-    [-126, 126] makes every element NaN.  ``out``: as in dequantize_fp8.  Asynchronous on the current stream."""
-    torch = _torch()
-    code = _operand(q, "q", _fp8_format)
-    dtype, dst = _float_dtype(dtype)
-    _one_element(scale_exp, torch.int32, q, "scale_exp")
-    out = _out(out, dtype, q)
-    with torch.cuda.device(q.device):
-        check(lib.b200va_dequantize_fp8_auto(code, q.data_ptr(), dst, out.data_ptr(), q.numel(), scale_exp.data_ptr(),
-                                             _stream_ptr(stream)), "b200va_dequantize_fp8_auto")
-    return out
+def _amax(amax, a):
+    """``amax``: None, or checked to be a one-element float64 tensor on a's device."""
+    return amax if amax is None else _one_element(amax, _torch().float64, a, "amax")
 
 
 def _matrix(a) -> tuple[int, int, int]:
@@ -305,6 +232,92 @@ def _out_shaped(out, dtype, shape, a, name: str):
     return out
 
 
+def _quantize(a, fmt, k: int, amax, out, stream, *, transpose=False, out_t=None, auto=False, scale_exp=None):
+    """The four per-tensor quantize wrappers: ``a`` of any shape, or with ``transpose`` the 2-D ``a`` whose transposed
+    bytes go to ``out_t``.  ``k`` is the host's scale exponent, or with ``auto`` the margin of one chosen on the device
+    and written to ``scale_exp`` (a new one when None), a None ``amax`` then being a zeroed one made on the call's
+    stream.  Returns out, then out_t when transposing, then scale_exp when auto."""
+    torch = _torch()
+    if transpose:
+        src, rows, cols = _matrix(a)
+    else:
+        src = _operand(a, "a")
+    dtype, code = _fp8_format(fmt)
+    if transpose:
+        out = _out_shaped(out, dtype, (rows, cols), a, "out")
+        out_t = _out_shaped(out_t, dtype, (cols, rows), a, "out_t")
+    else:
+        out = _out(out, dtype, a)
+    _amax(amax, a)
+    if auto:
+        scale_exp = (torch.empty(1, dtype=torch.int32, device=a.device) if scale_exp is None
+                     else _one_element(scale_exp, torch.int32, a, "scale_exp"))
+    name = "b200va_quantize_fp8" + "_transpose" * transpose + "_auto" * auto
+    shape = (out_t.data_ptr(), rows, cols) if transpose else (a.numel(),)
+    with torch.cuda.device(a.device):
+        st = stream if stream is not None else torch.cuda.current_stream()
+        if auto and amax is None:
+            with torch.cuda.stream(st):
+                amax = torch.zeros(1, dtype=torch.float64, device=a.device)
+        scale = (int(k), amax.data_ptr() if amax is not None else None) + ((scale_exp.data_ptr(),) if auto else ())
+        check(getattr(lib, name)(src, a.data_ptr(), code, out.data_ptr(), *shape, *scale, st.cuda_stream), name)
+    outs = (out, out_t) if transpose else (out,)
+    return outs + (scale_exp,) if auto else outs
+
+
+def _dequantize(q, name: str, dtype, out, stream, *, k: int = 0, auto=False, scale_exp=None):
+    """The two per-tensor dequantize wrappers: FP8 ``q`` (the argument ``name``) by the host's scale exponent ``k``,
+    or with ``auto`` by the one the device reads from ``scale_exp``."""
+    torch = _torch()
+    code = _operand(q, name, _fp8_format)
+    dtype, dst = _float_dtype(dtype)
+    if auto:
+        _one_element(scale_exp, torch.int32, q, "scale_exp")
+    out = _out(out, dtype, q)
+    fn = "b200va_dequantize_fp8_auto" if auto else "b200va_dequantize_fp8"
+    with torch.cuda.device(q.device):
+        check(getattr(lib, fn)(code, q.data_ptr(), dst, out.data_ptr(), q.numel(),
+                               scale_exp.data_ptr() if auto else int(k), _stream_ptr(stream)), fn)
+    return out
+
+
+def quantize_fp8(a, fmt, *, scale_exp: int = 0, amax=None, out=None, stream=None):
+    """``a`` (f32/f64/f16/bf16) times 2^scale_exp, rounded once to FP8 (b200va_quantize_fp8): round-to-nearest-even,
+    saturating at +-max finite (448 for E4M3, 57344 for E5M2), inf included; NaN stays NaN.  ``fmt``:
+    torch.float8_e4m3fn / torch.float8_e5m2 or "e4m3" / "e5m2".  ``amax``: a one-element float64 CUDA tensor that
+    max-accumulates max |a| (unscaled; NaN if any element is); set it to 0 before the first call.  ``out``: a
+    contiguous CUDA tensor of the FP8 dtype with a's length on a's device, else a new one.  Asynchronous on the
+    current stream."""
+    return _quantize(a, fmt, scale_exp, amax, out, stream)[0]
+
+
+def dequantize_fp8(a, dtype, *, scale_exp: int = 0, out=None, stream=None):
+    """FP8 ``a`` (torch.float8_e4m3fn / float8_e5m2) times 2^-scale_exp, rounded once to ``dtype``
+    (torch.float32/float64/float16/bfloat16, or "f32"/"f64"/"f16"/"bf16") by b200va_dequantize_fp8: round-to-nearest-
+    even, no FTZ, overflow to inf.  ``out``: a contiguous CUDA tensor of ``dtype`` with a's length on a's device, else
+    a new one.  Asynchronous on the current stream."""
+    return _dequantize(a, "a", dtype, out, stream, k=scale_exp)
+
+
+def quantize_fp8_auto(a, fmt, *, margin: int = 0, amax=None, scale_exp=None, out=None, stream=None):
+    """``a`` (f32/f64/f16/bf16) quantized to FP8 with a power-of-two scale 2^k chosen on the device from the amax
+    (b200va_quantize_fp8_auto): an amax pass max-accumulates the largest finite |a| into ``amax``, then k is the
+    largest exponent with amax 2^k <= max finite (448 for E4M3, 57344 for E5M2), less ``margin`` (0..126), clamped to
+    [-126, 126], and a[i] 2^k is rounded once by quantize_fp8's rules.  With margin >= 0, only +-inf saturates.
+    ``amax``: a one-element float64 CUDA tensor, the caller's running max; None makes a zeroed one on the stream
+    (current scaling).  ``scale_exp``: a one-element int32 CUDA tensor that receives k, else a new one.  ``out``: as
+    in quantize_fp8.  Returns (out, scale_exp) without a host sync; torch.exp2(-scale_exp.float()) is the per-tensor
+    dequantization scale a tensor-wise torch._scaled_mm takes.  Asynchronous on the current stream."""
+    return _quantize(a, fmt, margin, amax, out, stream, auto=True, scale_exp=scale_exp)
+
+
+def dequantize_fp8_auto(q, scale_exp, dtype, *, out=None, stream=None):
+    """FP8 ``q`` times 2^-k, k the one-element int32 CUDA tensor ``scale_exp`` that quantize_fp8_auto wrote, rounded
+    once to ``dtype`` by dequantize_fp8's rules (b200va_dequantize_fp8_auto); k is read on the device, and one outside
+    [-126, 126] makes every element NaN.  ``out``: as in dequantize_fp8.  Asynchronous on the current stream."""
+    return _dequantize(q, "q", dtype, out, stream, auto=True, scale_exp=scale_exp)
+
+
 def quantize_fp8_transpose(a, fmt, *, scale_exp: int = 0, amax=None, out=None, out_t=None, stream=None):
     """The 2-D ``a`` (rows x cols, contiguous, f32/f64/f16/bf16) quantized to FP8 as quantize_fp8 does, and the
     transpose of the result, in one pass over a (b200va_quantize_fp8_transpose).  ``out`` ([rows, cols]) gets the bytes
@@ -316,18 +329,7 @@ def quantize_fp8_transpose(a, fmt, *, scale_exp: int = 0, amax=None, out=None, o
     the weight gradient dW = dY^T X is ``torch._scaled_mm(dy_t, x_t.t(), scale_a, scale_b)`` with
     ``dy_t = quantize_fp8_transpose(dy, ...)[1]`` and ``x_t = quantize_fp8_transpose(x, ...)[1]``: x_t.t() is the
     column-major mat2 it requires, with no copy.  Asynchronous on the current stream."""
-    torch = _torch()
-    src, rows, cols = _matrix(a)
-    dtype, code = _fp8_format(fmt)
-    out = _out_shaped(out, dtype, (rows, cols), a, "out")
-    out_t = _out_shaped(out_t, dtype, (cols, rows), a, "out_t")
-    if amax is not None:
-        _one_element(amax, torch.float64, a, "amax")
-    with torch.cuda.device(a.device):
-        check(lib.b200va_quantize_fp8_transpose(src, a.data_ptr(), code, out.data_ptr(), out_t.data_ptr(), rows, cols,
-                                                int(scale_exp), amax.data_ptr() if amax is not None else None,
-                                                _stream_ptr(stream)), "b200va_quantize_fp8_transpose")
-    return out, out_t
+    return _quantize(a, fmt, scale_exp, amax, out, stream, transpose=True, out_t=out_t)
 
 
 def quantize_fp8_transpose_auto(a, fmt, *, margin: int = 0, amax=None, scale_exp=None, out=None, out_t=None,
@@ -337,24 +339,7 @@ def quantize_fp8_transpose_auto(a, fmt, *, margin: int = 0, amax=None, scale_exp
     in quantize_fp8_auto, ``out`` and ``out_t`` as in quantize_fp8_transpose.  Returns (out, out_t, scale_exp) without
     a host sync; torch.exp2(-scale_exp.float()) is the scale torch._scaled_mm takes for out or out_t.t().
     Asynchronous on the current stream."""
-    torch = _torch()
-    src, rows, cols = _matrix(a)
-    dtype, code = _fp8_format(fmt)
-    out = _out_shaped(out, dtype, (rows, cols), a, "out")
-    out_t = _out_shaped(out_t, dtype, (cols, rows), a, "out_t")
-    if amax is not None:
-        _one_element(amax, torch.float64, a, "amax")
-    scale_exp = (torch.empty(1, dtype=torch.int32, device=a.device) if scale_exp is None
-                 else _one_element(scale_exp, torch.int32, a, "scale_exp"))
-    with torch.cuda.device(a.device):
-        st = stream if stream is not None else torch.cuda.current_stream()
-        if amax is None:
-            with torch.cuda.stream(st):
-                amax = torch.zeros(1, dtype=torch.float64, device=a.device)
-        check(lib.b200va_quantize_fp8_transpose_auto(src, a.data_ptr(), code, out.data_ptr(), out_t.data_ptr(), rows,
-                                                     cols, int(margin), amax.data_ptr(), scale_exp.data_ptr(),
-                                                     st.cuda_stream), "b200va_quantize_fp8_transpose_auto")
-    return out, out_t, scale_exp
+    return _quantize(a, fmt, margin, amax, out, stream, transpose=True, out_t=out_t, auto=True, scale_exp=scale_exp)
 
 
 _U64 = (1 << 64) - 1
@@ -392,14 +377,11 @@ def quantize_fp8_sr(a, fmt, *, seed: int, offset: int = 0, scale_exp: int = 0, a
     NaN.  ``fmt``: torch.float8_e4m3fn / torch.float8_e5m2 or "e4m3" / "e5m2".  ``amax``: as in quantize_fp8.
     ``out``: a contiguous CUDA tensor of the FP8 dtype with a's length on a's device, else a new one.  Asynchronous on
     the current stream."""
-    torch = _torch()
     _sr_source(a)
     dtype, code = _fp8_format(fmt)
     out = _out(out, dtype, a)
-    if amax is not None and (not isinstance(amax, torch.Tensor) or amax.dtype != torch.float64 or amax.numel() != 1
-                             or amax.device != a.device):
-        raise TypeError("amax must be a one-element float64 tensor on a's device")
-    with torch.cuda.device(a.device):
+    _amax(amax, a)
+    with _torch().cuda.device(a.device):
         check(lib.b200va_quantize_fp8_sr_f32(a.data_ptr(), code, out.data_ptr(), a.numel(), int(scale_exp),
                                              int(seed) & _U64, int(offset) & _U64,
                                              amax.data_ptr() if amax is not None else None, _stream_ptr(stream)),

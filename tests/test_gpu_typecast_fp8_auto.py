@@ -381,8 +381,8 @@ def test_stream_op_quantize_dequantize_stream_op_on_one_stream():
 
 # ------------------------------------------------------------------------------------------- trace
 def expected_amax_launch(kernel, es, n, a_ptr):
-    """(kernel, grid, block) of launch_fp8_amax (b200va_typed.cu): A alone, its vector body from the head that puts
-    A on a 16-byte boundary, a group of 16 per unit, every other element an edge item."""
+    """(kernel, grid, block) of the amax pass (plan_fp8_amax, b200va_typed.cu): A alone, its vector body from the head
+    that puts A on a 16-byte boundary, a group of 16 per unit, every other element an edge item."""
     head = min(((16 - a_ptr % 16) % 16) // es, n)
     ngroups = (n - head) // 16
     edges = n - 16 * ngroups

@@ -404,7 +404,7 @@ def test_captured_auto_graph_follows_the_scale_across_replays():
 
 # ------------------------------------------------------------------------------------------- trace
 def expected_transpose_launch(src, rows, cols, pa, pc, pt):
-    """(kernel, grid, block) of launch_fp8_transpose (b200va_typed.cu): 256 threads and one 64 x 64 tile per CTA on
+    """(kernel, grid, block) of plan_fp8_transpose (b200va_typed.cu): 256 threads and one 64 x 64 tile per CTA on
     the tiled path; else every element an edge item, 512 threads in A's HBM class and 256 below it."""
     n = rows * cols
     kernel = f"fp8_quant_vec<{DT_CODE[src]}>"
