@@ -411,6 +411,55 @@ int b200va_dequantize_mxfp8(int fp8, const void *dA, const void *dS, int dst_dty
 /* Scale bytes for n elements: ceil(n / block); 0 for n = 0 or a block that is not 32, 64 or 128. */
 size_t b200va_mxfp8_scale_bytes(size_t n, int block);
 
+/* ---- blockwise FP8 quantize and dequantize for H100 FP8 GEMMs (row f4) -------------------------------
+ * The block-scaled operands of the H100's FP8 GEMMs (cuBLASLt's sm_90 blockwise scaling, torch's
+ * ScalingType.BlockWise1x128 / BlockWise128x128): f32 scales, one per block of: */
+#define B200VA_FP8_BLOCK_1X128    0   /* one scale per row and 128 columns: activations, gradients */
+#define B200VA_FP8_BLOCK_128X128  1   /* one scale per 128 x 128 tile: weights                    */
+/* A is row-major rows x cols, contiguous, of any B200VA_DT_* type.  C is row-major rows x cols FP8 and Ct row-major
+ * cols x rows FP8 (the transposed operand); S and St hold their f32 scales.
+ * Blocks.  1x128 row-wise (C, S): block (i, b) is A[i, 128b .. min(cols, 128b + 128)).  1x128 column-wise (Ct, St):
+ * the 1x128 blocks of A^T, A[128b .. min(rows, 128b + 128), j].  128x128: block (p, q) is the tile
+ * A[128p .., 128q ..] clipped at the edges; Ct is then exactly the byte transpose of C and St the same scales in the
+ * transposed operand's layout.  The last block in each direction may be short.
+ * Scale rule.  m is the largest finite |a| in the block, widened exactly; NaN and +-inf do not take part (the MXFP8
+ * and _auto rule).  k = clamp(K(m), -126, 126), K(m) the largest k with m * 2^k <= max finite (448 / 57344),
+ * K(0) = +inf: an all-zero block, or one with no finite element, gets k = 126.  k is the negated
+ * B200VA_MX_SCALE_NOSAT exponent clamped to [-126, 126], and b200va_quantize_fp8_auto's k with margin 0.  The block's
+ * scale is the f32 2^-k -- the dequantization factor the GEMM multiplies by; exact and always a normal f32.  Each
+ * element is sat(RN(a * 2^k)) by exactly the rules of b200va_quantize_fp8: one rounding, the format's subnormals, no
+ * FTZ, +-max finite for overflow and +-inf, NaN stays NaN, signed zeros kept.  With k unclamped no finite element
+ * saturates.
+ * Scale layouts (the ones torch.nn.functional.scaled_mm checks).  For an R x K operand (C: R = rows, K = cols; Ct:
+ * R = cols, K = rows), with nkb = ceil(K / 128), and L4 = ceil(nkb / 4) * 4:
+ *   1x128    S[b * R + r] for block b of row r: MN-major, an [R, nkb] view with strides [1, R];
+ *   128x128  S[p * L4 + q] for tile (p, q), p down R and q along K: an [L4, ceil(R / 128)] view with strides
+ *            [1, L4]; the padding entries q >= nkb are not written.
+ * Outputs.  (dC, dS) and (dCt, dSt) are each both NULL or both non-NULL: row-wise only, column-wise only, or both.
+ * Dequantize: c = RN_dst(q * s), s the f32 scale of q's block in the quantize's layout for (rows, cols, block_kind);
+ * to dequantize Ct pass St and (cols, rows).  s may be any f32, not only a power of two (scales from other producers,
+ * such as amax / 448, dequantize correctly): the product is exact (an FP8 value has at most 4 significant bits) and
+ * rounded once to dst_dtype by b200va_convert's rules (RNE, no FTZ, overflow to +-inf).  A NaN, +-inf or 0 scale gives
+ * the IEEE product.
+ * Arguments, in this order: B200VA_ERR_VARIANT: bad dtype, FP8 code or block kind.  B200VA_ERR_INVALID: a pair with
+ * one pointer NULL, nothing requested (or NULL dA) with rows * cols > 0, rows * cols overflowing or above 2^40
+ * (dequantize: NULL dA, dS or dC with rows * cols > 0, or the size rule).  B200VA_ERR_ALIGN: dA (quantize) or dC
+ * (dequantize) not aligned to its element size, dS or dSt not 4-byte aligned.  B200VA_ERR_OVERLAP: any two of A, C,
+ * S, Ct and St meet, scale padding included (dequantize: C meets A or S).  A rejected call writes nothing;
+ * rows == 0 or cols == 0 launches nothing.
+ * Both calls are one launch each: asynchronous on `stream`, no allocation, synchronisation or memset; capturable in a
+ * CUDA graph.  Fast path: cols % 128 == 0, rows % 16 == 0 and A, C and Ct on 16-byte boundaries; it reads A once
+ * from HBM and writes each output byte and scale once.  Any other shape or placement gives the same bytes through a
+ * per-block path that is not tuned.  Dequantize's fast path: cols % 16 == 0, A and C on 16-byte boundaries. */
+/* f32 scales of a rows x cols operand: 1x128: rows * ceil(cols/128); 128x128: ceil(rows/128) * L4,
+ * L4 = ceil(ceil(cols/128) / 4) * 4.  The transposed operand's count is this with rows and cols swapped.
+ * 0 for rows == 0, cols == 0 or a bad kind. */
+size_t b200va_fp8_blockwise_scales(size_t rows, size_t cols, int block_kind);
+int b200va_quantize_fp8_blockwise(int src_dtype, const void *dA, int fp8, int block_kind, size_t rows, size_t cols,
+                                  void *dC, float *dS, void *dCt, float *dSt, void *stream);
+int b200va_dequantize_fp8_blockwise(int fp8, const void *dA, const float *dS, int block_kind, int dst_dtype,
+                                    void *dC, size_t rows, size_t cols, void *stream);
+
 /* ---- stochastic rounding from f32 (row f4) ------------------------------------------------------
  * Narrowing that keeps, in expectation, what round-to-nearest drops: an f32 value rounds to one of its two
  * neighbours in the destination with probability given by its position between them, so an update smaller than

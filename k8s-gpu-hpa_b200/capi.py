@@ -32,6 +32,7 @@ F8_E4M3, F8_E5M2 = 0, 1                    # b200va_quantize_fp8 / b200va_dequan
 F8 = {"e4m3": F8_E4M3, "e5m2": F8_E5M2}
 MX_SCALE = {"ocp": 0, "nosat": 1}          # b200va_quantize_mxfp8 scale rules (B200VA_MX_SCALE_*)
 MX_BLOCKS = (32, 64, 128)
+FP8_BLOCK = {"1x128": 0, "128x128": 1}     # b200va_quantize_fp8_blockwise block kinds (B200VA_FP8_BLOCK_*)
 DOT_LANES, DOT_CHUNK = 2048, 65536         # b200va_dot's lane count and chunk size (B200VA_DOT_*)
 VARIANTS = {"auto": K_AUTO, "k0": K0_SCALAR, "k1": K1_VEC128, "k2": K2_TMA, "k3": K3_VEC256}
 
@@ -122,6 +123,9 @@ _SIGS = {
     "b200va_quantize_mxfp8": (_I, [_I, _P, _I, _P, _P, _SZ, _I, _I, _P]),
     "b200va_dequantize_mxfp8": (_I, [_I, _P, _P, _I, _P, _SZ, _I, _P]),
     "b200va_mxfp8_scale_bytes": (_SZ, [_SZ, _I]),
+    "b200va_fp8_blockwise_scales": (_SZ, [_SZ, _SZ, _I]),
+    "b200va_quantize_fp8_blockwise": (_I, [_I, _P, _I, _I, _SZ, _SZ, _P, _P, _P, _P, _P]),
+    "b200va_dequantize_fp8_blockwise": (_I, [_I, _P, _P, _I, _I, _P, _SZ, _SZ, _P]),
     "b200va_convert_sr_f32": (_I, [_P, _I, _P, _SZ, _U64, _U64, _P]),
     "b200va_quantize_fp8_sr_f32": (_I, [_P, _I, _P, _SZ, _I, _U64, _U64, _P, _P]),
     "b200va_dot_workspace_bytes": (_SZ, [_SZ]),

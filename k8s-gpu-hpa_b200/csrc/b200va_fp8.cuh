@@ -115,10 +115,10 @@ __device__ __forceinline__ int auto_scale_exp(double m, int fmt, int margin)
     return min(max(K - margin, -126), 126);
 }
 
-// Elements e0 and e0 + 1 of the source words s, scaled by 2^k and rounded to two FP8 bytes (bits 0..15); m takes
-// their magnitudes.  With `one`, only e0 (the high byte is 0).
+// Elements e0 and e0 + 1 of the source words s, scaled by 2^k0 and 2^k1 and rounded to two FP8 bytes (bits 0..15); m
+// takes their magnitudes.  With `one`, only e0 (the high byte is 0).
 template <int SRC, int F8, bool ONE = false>
-__device__ __forceinline__ uint32_t quant_pair(const uint32_t* s, int e0, int k, amax_bits_t<SRC>& m)
+__device__ __forceinline__ uint32_t quant_pair(const uint32_t* s, int e0, int k0, int k1, amax_bits_t<SRC>& m)
 {
     float q[2] = {0.f, 0.f};
 #pragma unroll
@@ -126,14 +126,21 @@ __device__ __forceinline__ uint32_t quant_pair(const uint32_t* s, int e0, int k,
         if constexpr (SRC == DT_F64) {
             const double x = elem_f64(s, e0 + j);
             m = max(m, static_cast<unsigned long long>(__double_as_longlong(x)) & 0x7fffffffffffffffull);
-            q[j] = f32_round_odd(__dmul_rn(x, pow2<SRC>(k)));
+            q[j] = f32_round_odd(__dmul_rn(x, pow2<SRC>(j ? k1 : k0)));
         } else {
             const float x = elem_f32<SRC>(s, e0 + j);
             m = max(m, __float_as_uint(x) & 0x7fffffffu);
-            q[j] = __fmul_rn(x, pow2<SRC>(k));
+            q[j] = __fmul_rn(x, pow2<SRC>(j ? k1 : k0));
         }
     }
     return f8x2_from_f32<F8>(q[0], q[1]);
+}
+
+// The same with one scale exponent k for both elements.
+template <int SRC, int F8, bool ONE = false>
+__device__ __forceinline__ uint32_t quant_pair(const uint32_t* s, int e0, int k, amax_bits_t<SRC>& m)
+{
+    return quant_pair<SRC, F8, ONE>(s, e0, k, k, m);
 }
 
 // One group: the 16 elements in the source words s, scaled by 2^k and rounded to the 16 FP8 bytes of the words d; m

@@ -344,11 +344,12 @@ int launch_mx_typed(const void* dA, void* dS, void* dC, size_t n, int dt, int fm
         p.ngroups -= p.ngroups % per_block;
         plan_geometry(p, hbm_class(n, ES), p.ngroups, (n + block - 1) / block - p.ngroups / per_block);
         return launch_kernel(mx_quant_vec<ES>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dC, dS, n, p.ngroups, p.unroll,
-                             p.prefetch_first, dt, fmt, block, rule);
+                             p.prefetch_first, dt, fmt, block, rule, static_cast<void*>(nullptr), static_cast<void*>(nullptr),
+                             size_t{0}, size_t{0}, 0);
     } else {
         plan_geometry(p, hbm_class(n, ES), p.ngroups * ES, n - p.ngroups * 16);
         return launch_kernel(mx_dequant_vec<ES>, p.grid, p.threads, 0, st, pdl_enabled(), dA, dS, dC, n, p.ngroups, p.unroll,
-                             p.prefetch_first, dt, fmt, block);
+                             p.prefetch_first, dt, fmt, block, size_t{0}, size_t{0}, 0);
     }
 }
 
@@ -362,6 +363,62 @@ int check_mx_args(size_t es, const void* dA, size_t esc, const void* dC, const v
     RC_TRY(check_convert_operands(es, dA, esc, dC, n));
     const size_t sbytes = b200va_mxfp8_scale_bytes(n, block);
     if (ranges_meet(dS, sbytes, dA, n * es) || ranges_meet(dS, sbytes, dC, n * esc)) return B200VA_ERR_OVERLAP;
+    return B200VA_OK;
+}
+
+// rows cols, saturated at 2^40 + 1 when the product overflows, so that the operand checks reject it as n > 2^40.
+size_t matrix_elems(size_t rows, size_t cols)
+{
+    constexpr size_t past = (size_t{1} << 40) + 1;
+    return cols && rows > past / cols ? past : rows * cols;
+}
+
+// The blockwise quantize's plan, n = rows cols > 0 elements of es bytes, C and / or Ct requested.  The tiled path runs
+// when cols % 128 == 0, rows % 16 == 0 and A, C and Ct (those requested) sit on 16-byte boundaries: ngroups = n / 16,
+// FP8B_THREADS threads, one CTA per 128 x 128 tile and FP8B_SMEM bytes of dynamic shared memory (smem).  Otherwise the
+// per-block path: ngroups = 0, one edge item per block (1 x 128: C's blocks, then Ct's; 128 x 128: one per tile) under
+// plan_geometry for A's HBM class.  Neither prefetches a first tile, and neither geometry was tuned.
+cast_plan plan_fp8_blockwise(uintptr_t a, uintptr_t c, uintptr_t ct, size_t es, size_t rows, size_t cols, int kind,
+                             size_t& smem)
+{
+    constexpr size_t T = FP8B_TILE;
+    const size_t n = rows * cols, nkb_r = (rows + T - 1) / T, nkb_c = (cols + T - 1) / T;
+    cast_plan p{};
+    smem = 0;
+    if (cols % T == 0 && rows % 16 == 0 && ((a | c | ct) & 15u) == 0) {
+        p.ngroups = n / 16;
+        p.threads = FP8B_THREADS;
+        p.unroll = 1;
+        p.grid = static_cast<unsigned>(std::min<size_t>(nkb_r * nkb_c, 0x7fffffff));
+        smem = FP8B_SMEM;
+    } else {
+        const size_t items = kind == FP8B_1X128 ? (c ? rows * nkb_c : 0) + (ct ? cols * nkb_r : 0) : nkb_r * nkb_c;
+        plan_geometry(p, hbm_class(n, es), 0, items);
+        p.prefetch_first = 0;
+    }
+    return p;
+}
+
+// The argument rules of b200va_quantize_fp8_blockwise after the dtype, format and kind codes, in the order they
+// apply (A of es bytes per element, rows x cols; the caller has checked that the two pairs are each all-NULL or
+// all-non-NULL):
+//   1. with n = rows cols > 0: something requested, dA non-NULL, and n (saturated on overflow) at most 2^40;
+//   2. A aligned to its element size, S and St 4-byte aligned (C and Ct are bytes: any address);
+//   3. no two of A, C, S, Ct and St meeting, the scales' padding included.
+int check_fp8_blockwise_args(size_t es, const void* dA, const void* dC, const float* dS, const void* dCt,
+                             const float* dSt, size_t rows, size_t cols, int kind)
+{
+    const size_t n = matrix_elems(rows, cols);
+    if (n && ((!dC && !dCt) || !dA || n > (size_t{1} << 40))) return B200VA_ERR_INVALID;
+    if ((reinterpret_cast<uintptr_t>(dA) & (es - 1)) || (reinterpret_cast<uintptr_t>(dS) & 3u) ||
+        (reinterpret_cast<uintptr_t>(dSt) & 3u))
+        return B200VA_ERR_ALIGN;
+    const void* p[5] = {dA, dC, dS, dCt, dSt};
+    const size_t bytes[5] = {n * es, dC ? n : 0, dS ? 4 * b200va_fp8_blockwise_scales(rows, cols, kind) : 0,
+                             dCt ? n : 0, dSt ? 4 * b200va_fp8_blockwise_scales(cols, rows, kind) : 0};
+    for (int x = 0; x < 5; ++x)
+        for (int y = x + 1; y < 5; ++y)
+            if (ranges_meet(p[x], bytes[x], p[y], bytes[y])) return B200VA_ERR_OVERLAP;
     return B200VA_OK;
 }
 
@@ -487,6 +544,61 @@ int b200va_dequantize_mxfp8(int fp8, const void* dA, const void* dS, int dst_dty
     int rc = B200VA_ERR_VARIANT;
     with_value<4, 8, 2>(static_cast<int>(dtype_size(dst_dtype)), [&](auto ES) {
         rc = launch_mx_typed<false, ES>(dA, const_cast<void*>(dS), dC, n, dst_dtype, fp8, block, 0, static_cast<cudaStream_t>(stream));
+    });
+    return rc;
+}
+
+size_t b200va_fp8_blockwise_scales(size_t rows, size_t cols, int block_kind)
+{
+    constexpr size_t T = FP8B_TILE;
+    if (!rows || !cols || block_kind < 0 || block_kind >= FP8B_COUNT) return 0;
+    const size_t nkb_c = (cols + T - 1) / T;
+    return block_kind == FP8B_1X128 ? rows * nkb_c : (rows + T - 1) / T * ((nkb_c + 3) / 4 * 4);
+}
+
+int b200va_quantize_fp8_blockwise(int src_dtype, const void* dA, int fp8, int block_kind, size_t rows, size_t cols,
+                                  void* dC, float* dS, void* dCt, float* dSt, void* stream)
+{
+    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT || block_kind < 0 || block_kind >= FP8B_COUNT)
+        return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    if (!dC != !dS || !dCt != !dSt) return B200VA_ERR_INVALID;
+    const size_t es = dtype_size(src_dtype);
+    RC_TRY(check_fp8_blockwise_args(es, dA, dC, dS, dCt, dSt, rows, cols, block_kind));
+    if (rows == 0 || cols == 0) return B200VA_OK;
+    size_t smem = 0;
+    const cast_plan p = plan_fp8_blockwise(reinterpret_cast<uintptr_t>(dA), reinterpret_cast<uintptr_t>(dC),
+                                           reinterpret_cast<uintptr_t>(dCt), es, rows, cols, block_kind, smem);
+    int rc = B200VA_ERR_VARIANT;
+    with_value<4, 8, 2>(static_cast<int>(es), [&](auto ES) {
+        rc = launch_kernel(mx_quant_vec<ES>, p.grid, p.threads, smem, static_cast<cudaStream_t>(stream), pdl_enabled(), dA,
+                           dC, static_cast<void*>(dS), rows * cols, p.ngroups, p.unroll, p.prefetch_first, src_dtype, fp8, 0,
+                           0, dCt, static_cast<void*>(dSt), rows, cols, block_kind);
+    });
+    return rc;
+}
+
+int b200va_dequantize_fp8_blockwise(int fp8, const void* dA, const float* dS, int block_kind, int dst_dtype, void* dC,
+                                    size_t rows, size_t cols, void* stream)
+{
+    if (dst_dtype < 0 || dst_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT || block_kind < 0 || block_kind >= FP8B_COUNT)
+        return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    const size_t es = dtype_size(dst_dtype), n = matrix_elems(rows, cols);
+    if (n && (!dA || !dS || !dC || n > (size_t{1} << 40))) return B200VA_ERR_INVALID;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC);
+    if ((c & (es - 1)) || (reinterpret_cast<uintptr_t>(dS) & 3u)) return B200VA_ERR_ALIGN;
+    const size_t sbytes = 4 * b200va_fp8_blockwise_scales(rows, cols, block_kind);
+    if (ranges_meet(dC, n * es, dA, n) || ranges_meet(dC, n * es, dS, sbytes)) return B200VA_ERR_OVERLAP;
+    if (n == 0) return B200VA_OK;
+    cast_plan p{};
+    if (cols % 16 == 0 && ((a | c) & 15u) == 0) p.ngroups = n / 16;
+    plan_geometry(p, hbm_class(n, es), p.ngroups * es, n - p.ngroups * 16);
+    int rc = B200VA_ERR_VARIANT;
+    with_value<4, 8, 2>(static_cast<int>(es), [&](auto ES) {
+        rc = launch_kernel(mx_dequant_vec<ES>, p.grid, p.threads, 0, static_cast<cudaStream_t>(stream), pdl_enabled(), dA,
+                           static_cast<const void*>(dS), dC, n, p.ngroups, p.unroll, p.prefetch_first, dst_dtype, fp8, 0,
+                           rows, cols, block_kind);
     });
     return rc;
 }

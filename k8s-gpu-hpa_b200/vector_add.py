@@ -444,6 +444,94 @@ def dequantize_mxfp8(q, scales, dtype, *, block: int = 32, out=None, stream=None
     return out
 
 
+def fp8_blockwise_scale_layout(rows: int, cols: int, block: str) -> tuple[int, tuple[int, int], tuple[int, int]]:
+    """(numel, shape, stride) of the f32 scales of a rows x cols operand quantized in ``block`` ("1x128" or
+    "128x128") blocks: the storage b200va_quantize_fp8_blockwise writes, and the as_strided view of it that
+    torch.nn.functional.scaled_mm takes (MN-major).  1x128: S[b * rows + i], an [rows, ceil(cols/128)] view with strides
+    [1, rows].  128x128: S[p * L4 + q], an [L4, ceil(rows/128)] view with strides [1, L4], L4 = ceil(ceil(cols/128) / 4)
+    4 (the entries q >= ceil(cols/128) are padding).  The transposed operand's layout is this with rows and cols
+    swapped."""
+    if block not in capi.FP8_BLOCK:
+        raise ValueError(f"block must be one of {sorted(capi.FP8_BLOCK)}, got {block!r}")
+    nkb_r, nkb_c = -(-rows // 128), -(-cols // 128)
+    if block == "1x128":
+        return rows * nkb_c, (rows, nkb_c), (1, max(rows, 1))
+    l4 = -(-nkb_c // 4) * 4
+    return nkb_r * l4, (l4, nkb_r), (1, l4)
+
+
+def _blockwise_scales(scales, rows: int, cols: int, block: str, dev, name: str):
+    """``scales`` checked to be a float32 tensor on ``dev`` whose storage holds the layout's count from its storage
+    offset, viewed in the layout; or a new one."""
+    torch = _torch()
+    numel, shape, stride = fp8_blockwise_scale_layout(rows, cols, block)
+    if scales is None:
+        return torch.empty(numel, dtype=torch.float32, device=dev).as_strided(shape, stride)
+    if (not isinstance(scales, torch.Tensor) or scales.dtype != torch.float32 or scales.device != dev
+            or scales.untyped_storage().nbytes() // 4 - scales.storage_offset() < numel):
+        raise TypeError(f"{name} must be a float32 tensor on {dev} with storage for {numel} scales")
+    return scales.as_strided(shape, stride)
+
+
+def quantize_fp8_blockwise(a, fmt, *, block: str = "1x128", rowwise: bool = True, columnwise: bool = True, out=None,
+                           scales=None, out_t=None, scales_t=None, stream=None):
+    """The 2-D ``a`` (rows x cols, contiguous, f32/f64/f16/bf16) quantized to FP8 with one f32 power-of-two scale per
+    block (b200va_quantize_fp8_blockwise), the operands of an H100 blockwise-scaled FP8 GEMM.  ``block``: "1x128"
+    (activations, gradients) or "128x128" (weights).  Per block, k is the largest exponent with amax 2^k <= max finite
+    (amax over the finite elements), clamped to [-126, 126]; the scale is 2^-k and each element a 2^k rounded once by
+    quantize_fp8's rules.  ``rowwise``: ``out`` ([rows, cols]) and ``scales`` in A's blocks; ``columnwise``: ``out_t``
+    ([cols, rows]) and ``scales_t`` in the blocks of A^T (for 1x128, 128 x 1 blocks of a along its columns); both in
+    one pass over a.  Returns (out, scales, out_t, scales_t), None for a side not asked for; each scale tensor is the
+    view fp8_blockwise_scale_layout gives, so ``out`` with ``scales`` and ``out_t.t()`` with ``scales_t`` go to
+    torch.nn.functional.scaled_mm as they are.  Asynchronous on the current stream."""
+    torch = _torch()
+    src, rows, cols = _matrix(a)
+    dtype, code = _fp8_format(fmt)
+    if block not in capi.FP8_BLOCK:
+        raise ValueError(f"block must be one of {sorted(capi.FP8_BLOCK)}, got {block!r}")
+    if not rowwise and not columnwise:
+        raise ValueError("at least one of rowwise and columnwise must be set")
+    if rowwise:
+        out = _out_shaped(out, dtype, (rows, cols), a, "out")
+        scales = _blockwise_scales(scales, rows, cols, block, a.device, "scales")
+    else:
+        out = scales = None
+    if columnwise:
+        out_t = _out_shaped(out_t, dtype, (cols, rows), a, "out_t")
+        scales_t = _blockwise_scales(scales_t, cols, rows, block, a.device, "scales_t")
+    else:
+        out_t = scales_t = None
+    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    with torch.cuda.device(a.device):
+        check(lib.b200va_quantize_fp8_blockwise(src, a.data_ptr(), code, capi.FP8_BLOCK[block], rows, cols, ptr(out),
+                                                ptr(scales), ptr(out_t), ptr(scales_t), _stream_ptr(stream)),
+              "b200va_quantize_fp8_blockwise")
+    return out, scales, out_t, scales_t
+
+
+def dequantize_fp8_blockwise(q, scales, dtype, *, block: str, out=None, stream=None):
+    """The 2-D FP8 ``q`` (rows x cols, torch.float8_e4m3fn / float8_e5m2) with its f32 block ``scales`` (the view
+    quantize_fp8_blockwise returns, or any float32 tensor whose storage holds the layout) back to ``dtype``
+    (b200va_dequantize_fp8_blockwise): q s rounded once, s the scale of q's block, any f32 (not only a power of two).
+    For ``out_t`` pass ``scales_t``.  ``out``: a contiguous [rows, cols] tensor of ``dtype`` on q's device, else a new
+    one.  Asynchronous on the current stream."""
+    torch = _torch()
+    code = _operand(q, "q", _fp8_format)
+    if q.dim() != 2:
+        raise TypeError(f"q must be a 2-D tensor, got {q.dim()} dimensions")
+    rows, cols = q.shape
+    dtype, dst = _float_dtype(dtype)
+    if scales is None:
+        raise TypeError("scales must be given")
+    scales = _blockwise_scales(scales, rows, cols, block, q.device, "scales")
+    out = _out_shaped(out, dtype, (rows, cols), q, "out")
+    with torch.cuda.device(q.device):
+        check(lib.b200va_dequantize_fp8_blockwise(code, q.data_ptr(), scales.data_ptr(), capi.FP8_BLOCK[block], dst,
+                                                  out.data_ptr(), rows, cols, _stream_ptr(stream)),
+              "b200va_dequantize_fp8_blockwise")
+    return out
+
+
 def dot(a, b, *, out=None, workspace=None, stream=None):
     """The reproducible dot product of two equal-length contiguous CUDA tensors of one of f32/f64/f16/bf16
     (b200va_dot): a 0-d float64 CUDA tensor, written asynchronously on the current stream.  The bits

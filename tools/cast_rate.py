@@ -1,6 +1,7 @@
 """Rate of the cast kernels by family, next to the f32 COPY and READ2 ceiling probes, in one process.
 
-    python tools/cast_rate.py [--family convert|fp8|fp8t|mxfp8|sr|all] [--log2n 28] [--calls 20] [--rounds 3]
+    python tools/cast_rate.py [--family convert|fp8|fp8t|fp8b|mxfp8|sr|all] [--log2n 28] [--calls 20] [--rounds 3]
+                              [--shape ROWSxCOLS]
 
 Per round, every op of the chosen families is timed at n elements with CUDA events around `calls` back-to-back calls
 (after two warm-up calls), then b200va_probe_f32 COPY (8 n bytes) and READ2 (8 n read) at the same n.  The families
@@ -19,6 +20,12 @@ and the algorithmic bytes of one call:
            C), the same followed by torch's transpose of the FP8 result into a preallocated tensor, the _auto form,
            and b200va_quantize_fp8_auto followed by torch's transpose.  Every entry counts n * (sizeof T + 2) bytes,
            what the fused call moves, so the rates compare times.
+  fp8b     the blockwise quantize at FP8T_SHAPES (or --shape) from each type to E4M3, and to E5M2 at 8192 x 8192:
+           1x128 with both sides, row-wise only and column-wise only, and 128x128 with Ct; beside them at the same
+           shape the quantize-transpose (the same bytes less the scales), quantize_mxfp8 at block 128 on the flattened
+           A (the yardstick of the row-wise-only case), and the torch-eager recipe for both 1x128 sides (view as
+           blocks, amax, exp2 of the scale exponent, multiply, .to(float8); .t().contiguous() and the same again).
+           Each entry counts n (sizeof T + outputs) + 4 (scale floats) bytes for what it writes.
   mxfp8    per type and format, alternated in this order: quantize and dequantize at block 32 and at block 128,
            n * (sizeof T + 1 + 1 / block); the per-tensor recipes they compete with are in the fp8 family.
   sr       the stochastically rounding casts from f32, each beside its round-to-nearest counterpart: to f16 and bf16,
@@ -138,6 +145,52 @@ def fp8t_ops(torch, va, n, tdt, f8):
             del a, amax, k
 
 
+def fp8b_ops(torch, va, n, tdt, f8, shapes=FP8T_SHAPES):
+    """n is unused: the blockwise family runs at FP8T_SHAPES (or the --shape given)."""
+    for rows, cols in shapes:
+        m = rows * cols
+        ns, nst = m // 128, m // 128                                    # 1x128 scales of each side
+        for s in tdt:
+            a = torch.randn(rows, cols, dtype=torch.float32, device="cuda").to(tdt[s])
+            for f in (("e4m3", "e5m2") if (rows, cols) == (8192, 8192) else ("e4m3",)):
+                q = torch.empty(rows, cols, dtype=f8[f], device="cuda")
+                qt = torch.empty(cols, rows, dtype=f8[f], device="cuda")
+                sc = torch.empty(ns, dtype=torch.float32, device="cuda")
+                sct = torch.empty(nst, dtype=torch.float32, device="cuda")
+                s128 = torch.empty(va.fp8_blockwise_scale_layout(rows, cols, "128x128")[0], dtype=torch.float32, device="cuda")
+                s128t = torch.empty(va.fp8_blockwise_scale_layout(cols, rows, "128x128")[0], dtype=torch.float32, device="cuda")
+                e8 = torch.empty(ns, dtype=torch.uint8, device="cuda")
+                top = 448.0 if f == "e4m3" else 57344.0
+                tag = f"{s}->{f} {rows}x{cols}"
+
+                def eager_side(x):
+                    blocks = x.float().reshape(x.shape[0], -1, 128)
+                    amax = blocks.abs().nan_to_num(0.0, 0.0, 0.0).amax(dim=2, keepdim=True)
+                    k = torch.floor(torch.log2(top / amax)).clamp(-126, 126)
+                    return (blocks * torch.exp2(k)).to(f8[f]).reshape(x.shape), torch.exp2(-k).squeeze(2).t().contiguous()
+
+                def eager():
+                    eager_side(a)
+                    eager_side(a.t().contiguous())
+
+                both = m * (SIZE[s] + 2) + 4 * (ns + nst)
+                yield (f"fp8 blockwise 1x128 both {tag}",
+                       lambda: va.quantize_fp8_blockwise(a, f8[f], out=q, scales=sc, out_t=qt, scales_t=sct), both)
+                yield (f"fp8 blockwise 1x128 rowwise {tag}",
+                       lambda: va.quantize_fp8_blockwise(a, f8[f], columnwise=False, out=q, scales=sc), m * (SIZE[s] + 1) + 4 * ns)
+                yield (f"fp8 blockwise 1x128 columnwise {tag}",
+                       lambda: va.quantize_fp8_blockwise(a, f8[f], rowwise=False, out_t=qt, scales_t=sct), m * (SIZE[s] + 1) + 4 * nst)
+                yield (f"fp8 blockwise 128x128 both {tag}",
+                       lambda: va.quantize_fp8_blockwise(a, f8[f], block="128x128", out=q, scales=s128, out_t=qt, scales_t=s128t),
+                       m * (SIZE[s] + 2) + 4 * (s128.numel() + s128t.numel()))
+                yield (f"quantize_fp8_transpose {tag}", lambda: va.quantize_fp8_transpose(a, f8[f], out=q, out_t=qt), both)
+                yield (f"quantize_mxfp8 block 128 {tag}",
+                       lambda: va.quantize_mxfp8(a.view(-1), f8[f], block=128, out=q.view(-1), scales=e8), m * (SIZE[s] + 1) + ns)
+                yield f"torch eager 1x128 both {tag}", eager, both
+                del q, qt, sc, sct, s128, s128t, e8
+            del a
+
+
 def mxfp8_ops(torch, va, n, tdt, f8):
     for s in tdt:
         a = torch.randn(n, dtype=torch.float32, device="cuda").to(tdt[s])
@@ -183,7 +236,7 @@ def sr_ops(torch, va, n, tdt, f8):
     del a, amax, c
 
 
-FAMILIES = {"convert": convert_ops, "fp8": fp8_ops, "fp8t": fp8t_ops, "mxfp8": mxfp8_ops, "sr": sr_ops}
+FAMILIES = {"convert": convert_ops, "fp8": fp8_ops, "fp8t": fp8t_ops, "fp8b": fp8b_ops, "mxfp8": mxfp8_ops, "sr": sr_ops}
 
 
 def main() -> None:
@@ -192,6 +245,7 @@ def main() -> None:
     ap.add_argument("--log2n", type=int, default=28)
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--shape", default=None, help="ROWSxCOLS: run the fp8b family at this shape only")
     args = ap.parse_args()
 
     import torch
@@ -212,7 +266,11 @@ def main() -> None:
 
     for r in range(args.rounds):
         for family in families:
-            for op, fn, nbytes in FAMILIES[family](torch, va, n, tdt, f8):
+            ops = FAMILIES[family]
+            if family == "fp8b" and args.shape:
+                shape = tuple(int(v) for v in args.shape.split("x"))
+                ops = lambda *x: fp8b_ops(*x, shapes=(shape,))  # noqa: E731
+            for op, fn, nbytes in ops(torch, va, n, tdt, f8):
                 report(r, op, timed(fn, args.calls), nbytes)
         x, y, z = (torch.ones(n, dtype=torch.float32, device="cuda") for _ in range(3))
         for kind, nbytes in (("copy", 8 * n), ("read2", 8 * n)):
