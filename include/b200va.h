@@ -460,6 +460,46 @@ int b200va_quantize_fp8_blockwise(int src_dtype, const void *dA, int fp8, int bl
 int b200va_dequantize_fp8_blockwise(int fp8, const void *dA, const float *dS, int block_kind, int dst_dtype,
                                     void *dC, size_t rows, size_t cols, void *stream);
 
+/* ---- row-wise FP8 quantize and dequantize for H100 FP8 GEMMs (row f4) --------------------------------
+ * The operands of torch's ScalingType.RowWise scaled_mm (cuBLASLt's sm_90 outer-vector scaling): one f32 scale per
+ * row of each operand.  A is row-major rows x cols, contiguous, of any B200VA_DT_* type.  C is row-major rows x cols
+ * FP8 and S holds rows f32 scales; Ct is row-major cols x rows FP8 (the transposed operand) and St holds cols f32
+ * scales.  (dC, dS) and (dCt, dSt) are each both NULL or both non-NULL: row-wise only, column-wise only, or both.
+ * Scale rule.  The blockwise rule above with one block per row (C) or per column (Ct): m is the largest finite |a| of
+ * the row, widened exactly (NaN and +-inf do not take part); k = clamp(K(m), -126, 126) with _auto's margin-0 K, and
+ * k = 126 for an all-zero row or one with no finite element; the stored scale is the f32 2^-k; each element is
+ * sat(RN(a * 2^k)) by exactly the rules of b200va_quantize_fp8.  This is the power-of-two row-wise scale (448 / amax
+ * rounded down to a power of two) with the library's clamp.  S[r] is the largest of the row's 1x128 block scales.
+ * Scale layout.  S and St are plain f32 vectors: S viewed as [rows, 1] is scaled_mm's scale_a and St viewed as
+ * [1, cols] its scale_b (and S as [1, rows] when C is the second operand).  A linear layer Y = X W^T takes:
+ *   forward          Y  = X W^T    (C_X, S_X)   x (C_W^T, S_W)
+ *   data gradient    dX = dY W     (C_dY, S_dY) x (Ct_W^T, St_W)
+ *   weight gradient  dW = dY^T X   (Ct_dY, St_dY) x (Ct_X^T, St_X)
+ * so one call per tensor, both sides requested, makes everything that tensor contributes.
+ * Workspace.  d_work is caller-owned scratch of at least b200va_fp8_rowwise_workspace(rows, cols) bytes; its contents
+ * before and after the call are unspecified.  The call allocates nothing and needs no memset.
+ * Arguments, in this order: B200VA_ERR_VARIANT: bad dtype or FP8 code.  B200VA_ERR_INVALID: a pair with one pointer
+ * NULL; with rows * cols > 0, nothing requested, NULL dA, rows * cols overflowing or above 2^40, NULL d_work or
+ * work_bytes below the workspace size.  B200VA_ERR_ALIGN: dA not aligned to its element size, dS, dSt or d_work not
+ * 4-byte aligned.  B200VA_ERR_OVERLAP: any two of A, C, S, Ct, St and the workspace meet.  A rejected call writes
+ * nothing, the workspace included; rows == 0 or cols == 0 launches nothing.
+ * Quantize is three launches chained by programmatic dependent launch (the 1x128 block maxima of the requested sides
+ * into the workspace, their reduction to S and St, the cast), asynchronous on `stream` and capturable in a CUDA graph.
+ * Fast path: cols % 128 == 0, rows % 16 == 0 and A, C and Ct on 16-byte boundaries; it reads A twice (the second
+ * time mostly from HBM) and writes each output byte and scale once.  Any other shape or placement gives the same
+ * bytes through a path that is not tuned.
+ * Dequantize: c = RN_dst(q * S[r]), one scale per row, S any f32 (not only a power of two): the product is exact and
+ * rounded once by b200va_convert's rules, as in b200va_dequantize_fp8_blockwise, whose argument rules it follows (S
+ * holds rows scales).  To dequantize Ct pass St and (cols, rows).  One launch; fast path: cols % 16 == 0, A and C on
+ * 16-byte boundaries. */
+/* Workspace bytes: 4 * (rows * ceil(cols/128) + cols * ceil(rows/128)); 0 for rows == 0 or cols == 0. */
+size_t b200va_fp8_rowwise_workspace(size_t rows, size_t cols);
+int b200va_quantize_fp8_rowwise(int src_dtype, const void *dA, int fp8, size_t rows, size_t cols,
+                                void *dC, float *dS, void *dCt, float *dSt,
+                                void *d_work, size_t work_bytes, void *stream);
+int b200va_dequantize_fp8_rowwise(int fp8, const void *dA, const float *dS, int dst_dtype,
+                                  void *dC, size_t rows, size_t cols, void *stream);
+
 /* ---- stochastic rounding from f32 (row f4) ------------------------------------------------------
  * Narrowing that keeps, in expectation, what round-to-nearest drops: an f32 value rounds to one of its two
  * neighbours in the destination with probability given by its position between them, so an update smaller than

@@ -126,6 +126,9 @@ _SIGS = {
     "b200va_fp8_blockwise_scales": (_SZ, [_SZ, _SZ, _I]),
     "b200va_quantize_fp8_blockwise": (_I, [_I, _P, _I, _I, _SZ, _SZ, _P, _P, _P, _P, _P]),
     "b200va_dequantize_fp8_blockwise": (_I, [_I, _P, _P, _I, _I, _P, _SZ, _SZ, _P]),
+    "b200va_fp8_rowwise_workspace": (_SZ, [_SZ, _SZ]),
+    "b200va_quantize_fp8_rowwise": (_I, [_I, _P, _I, _SZ, _SZ, _P, _P, _P, _P, _P, _SZ, _P]),
+    "b200va_dequantize_fp8_rowwise": (_I, [_I, _P, _P, _I, _P, _SZ, _SZ, _P]),
     "b200va_convert_sr_f32": (_I, [_P, _I, _P, _SZ, _U64, _U64, _P]),
     "b200va_quantize_fp8_sr_f32": (_I, [_P, _I, _P, _SZ, _I, _U64, _U64, _P, _P]),
     "b200va_dot_workspace_bytes": (_SZ, [_SZ]),

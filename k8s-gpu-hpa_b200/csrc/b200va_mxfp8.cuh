@@ -118,8 +118,8 @@ __device__ __forceinline__ void mx_quant_body(const unsigned char* a, unsigned c
 //   1 x 128    S[b rows + i] for block b of row i; St[b cols + j] for block b of column j
 //   128 x 128  S[p L4 + q] for tile (p, q), L4 = ceil(ceil(cols / 128) / 4) 4; St[q L4t + p], L4t from rows alike
 //
-// Tiled path (cols % 128 == 0, rows % 16 == 0, A, C and Ct on 16-byte boundaries): one 128 x 128 tile of A per CTA
-// turn, grid-strided, FP8B_THREADS threads.  Warp w, lane l takes group g = l % 8 (columns 16 g .. 16 g + 15) of tile
+// Tiled path (cols % 128 == 0, rows % 16 == 0, A, C and Ct on 16-byte boundaries): one 128 x 128 tile of A per CTA,
+// FP8B_THREADS threads.  Warp w, lane l takes group g = l % 8 (columns 16 g .. 16 g + 15) of tile
 // rows 32 s + 4 w + l / 8, s = 0..3; the bottom tile row may hold 16..112 rows, whole warps' rows dropping out.
 //   1 x 128     without Ct, one sweep: the row's maximum over the 8 lanes of its row (block_max), its scale and
 //               quant_group to C.  With Ct, sweep 1 loads each group once and takes the column maxima over the
@@ -135,6 +135,15 @@ __device__ __forceinline__ void mx_quant_body(const unsigned char* a, unsigned c
 // Per-block path (every other shape or placement): one thread per block, two passes of element loads (the maximum,
 // then the cast) -- the correctness path, not tuned, reading A once per block kind it writes.
 enum : int { FP8B_1X128 = 0, FP8B_128X128 = 1, FP8B_COUNT = 2 };
+// The row-wise cast (b200va_quantize_fp8_rowwise) is three launches of the same kernel, told apart by kind:
+//   FP8R_MAXIMA  the 1 x 128 block scales of the requested sides into the workspace, in the 1 x 128 layouts (W[b rows
+//                + i] for block b of row i, then W'[b cols + j] for block b of column j), no bytes: the 1 x 128 cast's
+//                sweep 1 (fp8b_tiles) or its per-block path without the cast.  C and Ct only say which sides.
+//   FP8R_REDUCE  S[i] = max_b W[b rows + i], St[j] = max_b W'[b cols + j] (fp8r_reduce).  K is monotone and the clamp
+//                commutes with min, so a row's k is the min of its blocks' k: its scale, the max of theirs.
+//   FP8R_ROWS    every element rounded with its row's k (C) and its column's k (Ct), k = 127 - (S bits >> 23); the
+//                dequantize's kind too, one scale per row.
+enum : int { FP8R_MAXIMA = FP8B_COUNT, FP8R_REDUCE, FP8R_ROWS };
 constexpr int FP8B_TILE = 128;
 constexpr int FP8B_THREADS = 256;
 // the byte tile, then the warps' column maxima (8 x 128 as f64 bits at most), then the 128 column exponents
@@ -179,10 +188,33 @@ __device__ __forceinline__ void fp8b_row(const uint32_t* v, amax_bits_t<SRC> gm,
     if (g == 0) *s = fp8b_scale(k);
 }
 
-// The tiled path, one format and one block kind.
+// Byte b of d (b = 0..15) is A's column 16 g + b at tile row i: into the byte tile, at tile row 16 g + b and row i of
+// its swizzled chunk.
+__device__ __forceinline__ void fp8b_put_t(unsigned char* tile, const uint32_t* d, unsigned i, unsigned g)
+{
+    unsigned char* col = tile + 16 * g * FP8B_TILE + 16 * ((i / 16) ^ g) + i % 16;
+#pragma unroll
+    for (int b = 0; b < 16; ++b) col[b * FP8B_TILE] = static_cast<unsigned char>(d[b / 4] >> (8 * (b % 4)));
+}
+
+// The byte tile to Ct's rows j0 .. j0 + 127, columns i0 .. i0 + tr: 8 lanes per 128-byte row.
+__device__ __forceinline__ void fp8b_store_t(const unsigned char* tile, unsigned char* ct, size_t rows, size_t i0,
+                                             size_t j0, unsigned tr)
+{
+#pragma unroll
+    for (int u = 0; u < FP8B_TILE * FP8B_TILE / 16 / FP8B_THREADS; ++u) {
+        const unsigned chunk = threadIdx.x + u * FP8B_THREADS, j = chunk / 8, h = chunk % 8;
+        if (16 * h < tr)
+            stg128_bits<ST_NA>(ct + (j0 + j) * rows + i0 + 16 * h,
+                               *reinterpret_cast<const u32x4*>(tile + j * FP8B_TILE + 16 * (h ^ (j / 16))));
+    }
+}
+
+// The tiled path, one format and one block kind.  With kind FP8R_MAXIMA (1 x 128 only) it is sweep 1 alone: the row
+// blocks' scales to sc when c is set, the column blocks' to sct when ct is set, and no bytes.
 template <int SRC, int F8, int KIND>
 __device__ __forceinline__ void fp8b_tiles(const unsigned char* a, unsigned char* c, float* sc, unsigned char* ct,
-                                           float* sct, const fp8b_shape& sh)
+                                           float* sct, const fp8b_shape& sh, int kind)
 {
     constexpr int ES = dt_traits<SRC>::size, T = FP8B_TILE;
     using M = amax_bits_t<SRC>;
@@ -192,116 +224,193 @@ __device__ __forceinline__ void fp8b_tiles(const unsigned char* a, unsigned char
     int* kcol = reinterpret_cast<int*>(fp8b_smem + T * T + 8 * T * 8);            // [T] column exponents
     const size_t rows = sh.rows, cols = sh.cols;
     const unsigned w = threadIdx.x / 32, l = threadIdx.x % 32, g = l % 8, r = 4 * w + l / 8;
-    // at most 2^36 / T tile columns (rows >= 16) and 2^40 / (16 T) tiles
-    const unsigned tiles_c = static_cast<unsigned>(sh.nkb_c), ntiles = static_cast<unsigned>(sh.nkb_r) * tiles_c;
-    for (unsigned t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const unsigned p = t / tiles_c, q = t % tiles_c;
-        const size_t i0 = static_cast<size_t>(p) * T, j0 = static_cast<size_t>(q) * T;
-        const unsigned tr = static_cast<unsigned>(min(rows - i0, size_t{T}));
-        M tm = 0, unused = 0;
-        // sweep 1: A's groups once
+    // one CTA per tile: the launch has as many CTAs as tiles, at most 2^40 / (16 T) = 2^29 (and at most 2^36 / T tile
+    // columns, rows >= 16)
+    const unsigned tiles_c = static_cast<unsigned>(sh.nkb_c), p = blockIdx.x / tiles_c, q = blockIdx.x % tiles_c;
+    const size_t i0 = static_cast<size_t>(p) * T, j0 = static_cast<size_t>(q) * T;
+    const unsigned tr = static_cast<unsigned>(min(rows - i0, size_t{T}));
+    M tm = 0, unused = 0;
+    // sweep 1: A's groups once
 #pragma unroll 1
-        for (int s = 0; s < 4; ++s) {
-            const unsigned i = 32 * s + r;
-            if (i >= tr) continue;                                                // whole warps (tr % 16 == 0)
-            const size_t e = (i0 + i) * cols + j0 + 16 * g;
-            uint32_t v[4 * ES];
-            unpack<ES>(ld_vecs<ES>(a + e * ES, 0).v, v);
-            M gm = 0;
+    for (int s = 0; s < 4; ++s) {
+        const unsigned i = 32 * s + r;
+        if (i >= tr) continue;                                                // whole warps (tr % 16 == 0)
+        const size_t e = (i0 + i) * cols + j0 + 16 * g;
+        uint32_t v[4 * ES];
+        unpack<ES>(ld_vecs<ES>(a + e * ES, 0).v, v);
+        M gm = 0;
 #pragma unroll
-            for (int x = 0; x < 16; ++x) gm = max(gm, finite_mag<SRC>(v, x));
-            if constexpr (KIND == FP8B_1X128) {
-                if (!ct) {
-                    fp8b_row<SRC, F8>(v, gm, c + e, sc + q * rows + i0 + i, g);
-                    continue;
-                }
-                // the column maxima over the warp's 4 rows, max-accumulated into the warp's own row of part
-#pragma unroll
-                for (int x = 0; x < 16; ++x) {
-                    M f = finite_mag<SRC>(v, x);
-                    f = max(f, __shfl_xor_sync(0xffffffffu, f, 8));
-                    f = max(f, __shfl_xor_sync(0xffffffffu, f, 16));
-                    if (l < 8) part[w * T + 16 * g + x] = s ? max(part[w * T + 16 * g + x], f) : f;
-                }
-            } else {
-                tm = max(tm, gm);
-            }
-        }
-        // the exponents the second sweep needs
-        int k = 0;
+        for (int x = 0; x < 16; ++x) gm = max(gm, finite_mag<SRC>(v, x));
         if constexpr (KIND == FP8B_1X128) {
-            if (!ct) continue;
-            if (l < 8 && 4 * w >= tr) {                       // a warp below the tile's rows adds nothing
-#pragma unroll
-                for (int x = 0; x < 16; ++x) part[w * T + 16 * g + x] = 0;
-            }
-            __syncthreads();
-            if (threadIdx.x < T) {
-                M m = part[threadIdx.x];
-#pragma unroll
-                for (int u = 1; u < 8; ++u) m = max(m, part[u * T + threadIdx.x]);
-                const int kx = fp8b_exponent<SRC, F8>(m);
-                kcol[threadIdx.x] = kx;
-                sct[p * cols + j0 + threadIdx.x] = fp8b_scale(kx);
-            }
-            __syncthreads();
-        } else {
-            tm = warp_max(tm);
-            if (l == 0) part[w] = tm;
-            __syncthreads();
-            M m = part[0];
-#pragma unroll
-            for (int u = 1; u < 8; ++u) m = max(m, part[u]);
-            k = fp8b_exponent<SRC, F8>(m);
-            if (threadIdx.x == 0) {
-                if (c) sc[p * sh.l4 + q] = fp8b_scale(k);
-                if (ct) sct[q * sh.l4t + p] = fp8b_scale(k);
-            }
-        }
-        // sweep 2: the groups again, rounded for Ct (and C for 128 x 128)
-#pragma unroll 1
-        for (int s = 0; s < 4; ++s) {
-            const unsigned i = 32 * s + r;
-            if (i >= tr) continue;
-            const size_t e = (i0 + i) * cols + j0 + 16 * g;
-            uint32_t v[4 * ES], d[4];
-            unpack<ES>(ld_vecs<ES>(a + e * ES, 0).v, v);
-            if constexpr (KIND == FP8B_1X128) {
-                const int* kc = kcol + 16 * g;                    // the 16 columns' exponents
-#pragma unroll
-                for (int x = 0; x < 4; ++x)
-                    d[x] = quant_pair<SRC, F8>(v, 4 * x, kc[4 * x], kc[4 * x + 1], unused) |
-                           (quant_pair<SRC, F8>(v, 4 * x + 2, kc[4 * x + 2], kc[4 * x + 3], unused) << 16);
-            } else {
-                quant_group<SRC, F8>(v, k, unused, d);
-                if (c) stg128_bits<ST_NA>(c + e, u32x4{d[0], d[1], d[2], d[3]});
-            }
-            if (ct) {
-                // byte b is A's column 16 g + b: tile row 16 g + b, at row i of its swizzled chunk
-                unsigned char* col = tile + 16 * g * T + 16 * ((i / 16) ^ g) + i % 16;
-#pragma unroll
-                for (int b = 0; b < 16; ++b) col[b * T] = static_cast<unsigned char>(d[b / 4] >> (8 * (b % 4)));
-            }
-            if constexpr (KIND == FP8B_1X128) {
+            if (kind == FP8R_MAXIMA) {
                 if (c) {
-                    M gm = 0;
-#pragma unroll
-                    for (int x = 0; x < 16; ++x) gm = max(gm, finite_mag<SRC>(v, x));
-                    fp8b_row<SRC, F8>(v, gm, c + e, sc + q * rows + i0 + i, g);
+                    const int kr = fp8b_exponent<SRC, F8>(block_max(gm, 8));
+                    if (g == 0) sc[q * rows + i0 + i] = fp8b_scale(kr);
                 }
+                if (!ct) continue;
+            } else if (!ct) {
+                fp8b_row<SRC, F8>(v, gm, c + e, sc + q * rows + i0 + i, g);
+                continue;
             }
-        }
-        __syncthreads();
-        if (!ct) continue;                                    // 128 x 128 without Ct: the barrier keeps part apart
-        // Ct's rows j0 .. j0 + 127, columns i0 .. i0 + tr: 8 lanes per 128-byte row
+            // the column maxima over the warp's 4 rows, max-accumulated into the warp's own row of part
 #pragma unroll
-        for (int u = 0; u < T * T / 16 / FP8B_THREADS; ++u) {
-            const unsigned chunk = threadIdx.x + u * FP8B_THREADS, j = chunk / 8, h = chunk % 8;
-            if (16 * h < tr)
-                stg128_bits<ST_NA>(ct + (j0 + j) * rows + i0 + 16 * h,
-                                   *reinterpret_cast<const u32x4*>(tile + j * T + 16 * (h ^ (j / 16))));
+            for (int x = 0; x < 16; ++x) {
+                M f = finite_mag<SRC>(v, x);
+                f = max(f, __shfl_xor_sync(0xffffffffu, f, 8));
+                f = max(f, __shfl_xor_sync(0xffffffffu, f, 16));
+                if (l < 8) part[w * T + 16 * g + x] = s ? max(part[w * T + 16 * g + x], f) : f;
+            }
+        } else {
+            tm = max(tm, gm);
         }
     }
+    // the exponents the second sweep needs
+    int k = 0;
+    if constexpr (KIND == FP8B_1X128) {
+        if (!ct) return;
+        if (l < 8 && 4 * w >= tr) {                       // a warp below the tile's rows adds nothing
+#pragma unroll
+            for (int x = 0; x < 16; ++x) part[w * T + 16 * g + x] = 0;
+        }
+        __syncthreads();
+        if (threadIdx.x < T) {
+            M m = part[threadIdx.x];
+#pragma unroll
+            for (int u = 1; u < 8; ++u) m = max(m, part[u * T + threadIdx.x]);
+            const int kx = fp8b_exponent<SRC, F8>(m);
+            kcol[threadIdx.x] = kx;
+            sct[p * cols + j0 + threadIdx.x] = fp8b_scale(kx);
+        }
+        __syncthreads();
+        if (kind == FP8R_MAXIMA) return;                  // sweep 1 only
+    } else {
+        tm = warp_max(tm);
+        if (l == 0) part[w] = tm;
+        __syncthreads();
+        M m = part[0];
+#pragma unroll
+        for (int u = 1; u < 8; ++u) m = max(m, part[u]);
+        k = fp8b_exponent<SRC, F8>(m);
+        if (threadIdx.x == 0) {
+            if (c) sc[p * sh.l4 + q] = fp8b_scale(k);
+            if (ct) sct[q * sh.l4t + p] = fp8b_scale(k);
+        }
+    }
+    // sweep 2: the groups again, rounded for Ct (and C for 128 x 128)
+#pragma unroll 1
+    for (int s = 0; s < 4; ++s) {
+        const unsigned i = 32 * s + r;
+        if (i >= tr) continue;
+        const size_t e = (i0 + i) * cols + j0 + 16 * g;
+        uint32_t v[4 * ES], d[4];
+        unpack<ES>(ld_vecs<ES>(a + e * ES, 0).v, v);
+        if constexpr (KIND == FP8B_1X128) {
+            const int* kc = kcol + 16 * g;                    // the 16 columns' exponents
+#pragma unroll
+            for (int x = 0; x < 4; ++x)
+                d[x] = quant_pair<SRC, F8>(v, 4 * x, kc[4 * x], kc[4 * x + 1], unused) |
+                       (quant_pair<SRC, F8>(v, 4 * x + 2, kc[4 * x + 2], kc[4 * x + 3], unused) << 16);
+        } else {
+            quant_group<SRC, F8>(v, k, unused, d);
+            if (c) stg128_bits<ST_NA>(c + e, u32x4{d[0], d[1], d[2], d[3]});
+        }
+        if (ct) fp8b_put_t(tile, d, i, g);
+        if constexpr (KIND == FP8B_1X128) {
+            if (c) {
+                M gm = 0;
+#pragma unroll
+                for (int x = 0; x < 16; ++x) gm = max(gm, finite_mag<SRC>(v, x));
+                fp8b_row<SRC, F8>(v, gm, c + e, sc + q * rows + i0 + i, g);
+            }
+        }
+    }
+    __syncthreads();
+    if (!ct) return;
+    fp8b_store_t(tile, ct, rows, i0, j0, tr);
+}
+
+// k from a scale 2^-k that FP8R_REDUCE left (a normal f32 power of two, k in [-126, 126]).
+__device__ __forceinline__ int fp8r_k(float s) { return 127 - static_cast<int>(__float_as_uint(s) >> 23); }
+
+// FP8R_ROWS on the tiled path: fp8b_tiles' tiles, threads and byte tile, one sweep (the k are known, no maxima).  Each
+// group is rounded with its row's k into C (quant_group) and with its 16 columns' k (kcol, from St) into the byte tile
+// (quant_pair).
+template <int SRC, int F8>
+__device__ __forceinline__ void fp8r_tiles(const unsigned char* a, unsigned char* c, const float* sc, unsigned char* ct,
+                                           const float* sct, const fp8b_shape& sh)
+{
+    constexpr int ES = dt_traits<SRC>::size, T = FP8B_TILE;
+    extern __shared__ __align__(16) unsigned char fp8b_smem[];
+    unsigned char* tile = fp8b_smem;
+    int* kcol = reinterpret_cast<int*>(fp8b_smem + T * T + 8 * T * 8);
+    const size_t rows = sh.rows, cols = sh.cols;
+    const unsigned w = threadIdx.x / 32, l = threadIdx.x % 32, g = l % 8, r = 4 * w + l / 8;
+    const unsigned tiles_c = static_cast<unsigned>(sh.nkb_c), p = blockIdx.x / tiles_c, q = blockIdx.x % tiles_c;
+    const size_t i0 = static_cast<size_t>(p) * T, j0 = static_cast<size_t>(q) * T;
+    const unsigned tr = static_cast<unsigned>(min(rows - i0, size_t{T}));
+    amax_bits_t<SRC> unused = 0;
+    if (ct) {
+        if (threadIdx.x < T) kcol[threadIdx.x] = fp8r_k(sct[j0 + threadIdx.x]);
+        __syncthreads();
+    }
+#pragma unroll 1
+    for (int s = 0; s < 4; ++s) {
+        const unsigned i = 32 * s + r;
+        if (i >= tr) continue;
+        const size_t e = (i0 + i) * cols + j0 + 16 * g;
+        uint32_t v[4 * ES], d[4];
+        unpack<ES>(ld_vecs<ES>(a + e * ES, 0).v, v);
+        if (ct) {
+            const int* kc = kcol + 16 * g;
+#pragma unroll
+            for (int x = 0; x < 4; ++x)
+                d[x] = quant_pair<SRC, F8>(v, 4 * x, kc[4 * x], kc[4 * x + 1], unused) |
+                       (quant_pair<SRC, F8>(v, 4 * x + 2, kc[4 * x + 2], kc[4 * x + 3], unused) << 16);
+            fp8b_put_t(tile, d, i, g);
+        }
+        if (c) {
+            quant_group<SRC, F8>(v, fp8r_k(sc[i0 + i]), unused, d);
+            stg128_bits<ST_NA>(c + e, u32x4{d[0], d[1], d[2], d[3]});
+        }
+    }
+    if (!ct) return;
+    __syncthreads();
+    fp8b_store_t(tile, ct, rows, i0, j0, tr);
+}
+
+// FP8R_ROWS on every other shape or placement: one thread per element of A, its byte to C and / or Ct (untuned).
+template <int SRC, int F8>
+__device__ __forceinline__ void fp8r_elems(const unsigned char* a, unsigned char* c, const float* sc, unsigned char* ct,
+                                           const float* sct, const fp8b_shape& sh)
+{
+    constexpr int ES = dt_traits<SRC>::size;
+    const size_t n = sh.rows * sh.cols;
+    const double rd = __drcp_rn(static_cast<double>(sh.cols));
+    cast_edges(n, n, n, [=](size_t e) {
+        size_t j;
+        const size_t i = fp8b_div(e, sh.cols, rd, j);
+        amax_bits_t<SRC> unused = 0;
+        if (c) c[e] = quant_elem<SRC, F8>(a + e * ES, fp8r_k(sc[i]), unused);
+        if (ct) ct[j * sh.rows + i] = quant_elem<SRC, F8>(a + e * ES, fp8r_k(sct[j]), unused);
+    });
+}
+
+// FP8R_REDUCE: one thread per row (S, when set), then per column (St, when set), walking its blocks' scales in the
+// workspace w; consecutive threads read consecutive entries.  The scales are positive normals, so their bit patterns
+// order as they do.
+__device__ __forceinline__ void fp8r_reduce(const float* w, float* s, float* st, const fp8b_shape& sh)
+{
+    const size_t nr = s ? sh.rows : 0, n = nr + (st ? sh.cols : 0);
+    const float* wt = w + sh.rows * sh.nkb_c;
+    cast_edges(n, n, n, [=](size_t t) {
+        const bool row = t < nr;
+        const size_t u = row ? t : t - nr, pitch = row ? sh.rows : sh.cols, nb = row ? sh.nkb_c : sh.nkb_r;
+        const float* p = (row ? w : wt) + u;
+        uint32_t m = 0;
+#pragma unroll 4
+        for (size_t b = 0; b < nb; ++b) m = max(m, __float_as_uint(p[b * pitch]));
+        (row ? s : st)[u] = __uint_as_float(m);
+    });
 }
 
 // A block of the per-block path: the h x w elements (h, w <= 128) of A from pa on, row pitch cols; its maximum, then
@@ -324,6 +433,7 @@ __device__ __forceinline__ void fp8b_rect(const unsigned char* pa, unsigned char
     const int k = fp8b_exponent<SRC, F8>(m);
     if (s) *s = fp8b_scale(k);
     if (st) *st = fp8b_scale(k);
+    if (!pc && !pct) return;
 #pragma unroll 1
     for (unsigned y = 0; y < h; ++y)
 #pragma unroll 1
@@ -335,10 +445,10 @@ __device__ __forceinline__ void fp8b_rect(const unsigned char* pa, unsigned char
 }
 
 // The per-block path: 1 x 128 gives C's blocks (row i, block b) as items [0, nrow) and Ct's (column j, block b) as
-// the next ncol; 128 x 128 gives one item per tile, writing both.
+// the next ncol; 128 x 128 gives one item per tile, writing both.  Without `bytes` (FP8R_MAXIMA) only the scales.
 template <int SRC, int F8>
 __device__ __forceinline__ void fp8b_blocks(const unsigned char* a, unsigned char* c, float* sc, unsigned char* ct,
-                                            float* sct, const fp8b_shape& sh, int kind)
+                                            float* sct, const fp8b_shape& sh, int kind, bool bytes = true)
 {
     constexpr int ES = dt_traits<SRC>::size;
     constexpr size_t B = FP8B_TILE;
@@ -359,21 +469,23 @@ __device__ __forceinline__ void fp8b_blocks(const unsigned char* a, unsigned cha
                        w = static_cast<unsigned>(tiles || along ? min(cols - j, B) : 1);
         float* s = tiles ? (c ? sc + u * sh.l4 + b : nullptr) : along ? sc + b * rows + u : nullptr;
         float* st = tiles ? (ct ? sct + b * sh.l4t + u : nullptr) : along ? nullptr : sct + b * cols + u;
-        fp8b_rect<SRC, F8>(a + (i * cols + j) * ES, (tiles || along) && c ? c + i * cols + j : nullptr,
-                           tiles ? (ct ? ct + j * rows + i : nullptr) : along ? nullptr : ct + j * rows + i, rows, cols,
-                           h, w, s, st);
+        fp8b_rect<SRC, F8>(a + (i * cols + j) * ES, bytes && (tiles || along) && c ? c + i * cols + j : nullptr,
+                           !bytes ? nullptr : tiles ? (ct ? ct + j * rows + i : nullptr) : along ? nullptr : ct + j * rows + i,
+                           rows, cols, h, w, s, st);
     });
 }
 
-// The blockwise quantize after the dependency wait: the tiled path when ngroups (= n / 16) is set, else the
-// per-block path.
+// The blockwise quantize, and the row-wise cast's launches, after the dependency wait: the tiled path when ngroups
+// (= n / 16) is set, else the per-block (or per-element) path.
 template <int SRC, int F8>
 __device__ __forceinline__ void fp8b_quant_body(const unsigned char* a, unsigned char* c, float* sc, unsigned char* ct,
                                                 float* sct, size_t ngroups, const fp8b_shape& sh, int kind)
 {
-    if (!ngroups) fp8b_blocks<SRC, F8>(a, c, sc, ct, sct, sh, kind);
-    else if (kind == FP8B_1X128) fp8b_tiles<SRC, F8, FP8B_1X128>(a, c, sc, ct, sct, sh);
-    else fp8b_tiles<SRC, F8, FP8B_128X128>(a, c, sc, ct, sct, sh);
+    if (!ngroups && kind == FP8R_ROWS) fp8r_elems<SRC, F8>(a, c, sc, ct, sct, sh);
+    else if (!ngroups) fp8b_blocks<SRC, F8>(a, c, sc, ct, sct, sh, kind == FP8R_MAXIMA ? FP8B_1X128 : kind, kind != FP8R_MAXIMA);
+    else if (kind == FP8R_ROWS) fp8r_tiles<SRC, F8>(a, c, sc, ct, sct, sh);
+    else if (kind == FP8B_128X128) fp8b_tiles<SRC, F8, FP8B_128X128>(a, c, sc, ct, sct, sh, kind);
+    else fp8b_tiles<SRC, F8, FP8B_1X128>(a, c, sc, ct, sct, sh, kind);
 }
 
 // The shape of a rows x cols blockwise cast, as the host's b200va_fp8_blockwise_scales counts it.
@@ -405,7 +517,9 @@ __device__ __forceinline__ void mx_with_pair(int dt, int fmt, F f)
 // convert_vec; the prefetch covers the CTA's first tile of the vector body.
 // With cols != 0 the kernel is b200va_quantize_fp8_blockwise's (fp8b_quant_body): A is rows x cols, S and St are
 // f32, Ct and St may be null (and C and S), kind is an FP8B_* code, and block and rule are unused; the launch gives
-// FP8B_THREADS threads and FP8B_SMEM bytes of dynamic shared memory on the tiled path, and no prefetch.
+// FP8B_THREADS threads and FP8B_SMEM bytes of dynamic shared memory on the tiled path, and no prefetch.  With an
+// FP8R_* kind it is one of b200va_quantize_fp8_rowwise's three launches; FP8R_REDUCE reads the workspace at A and
+// writes S to C and St to Ct.
 // The launch bounds keep the register count at the 1-D launches' occupancy (two 512-thread CTAs per SM, one for f64),
 // which the blockwise body alone would exceed.
 template <int ES>
@@ -421,6 +535,11 @@ mx_quant_vec(const void* A, void* C, void* S, size_t n, size_t ngroups, int unro
 
     if (cols) {
         const fp8b_shape sh = fp8b_make_shape(rows, cols);
+        if (kind == FP8R_REDUCE) {
+            fp8r_reduce(static_cast<const float*>(A), static_cast<float*>(C), static_cast<float*>(Ct), sh);
+            return;
+        }
+
         mx_with_pair<ES>(src, fmt, [=](auto SRC, auto F8) {
             fp8b_quant_body<SRC, F8>(a, c, static_cast<float*>(S), static_cast<unsigned char*>(Ct), static_cast<float*>(St),
                                      ngroups, sh, kind);
@@ -464,17 +583,19 @@ __device__ __forceinline__ u32x4 fp8b_dequant_slice(unsigned long long v, float 
 
 // The blockwise dequantize after the dependency wait: dequant_body's layout (the vector body when cols % 16 == 0 and
 // A and C sit on 16-byte boundaries, ngroups = n / 16; a slice then lies in one row and one block) with the f32 scale
-// of the block element e = i cols + j lies in: sf[(j / 128) rows + i] (1 x 128) or sf[(i / 128) L4 + j / 128].
+// of the block element e = i cols + j lies in: sf[(j / 128) rows + i] (1 x 128), sf[(i / 128) L4 + j / 128] (128 x 128)
+// or sf[i] (FP8R_ROWS).
 template <int F8, int DST>
 __device__ __forceinline__ void fp8b_dequant_body(const unsigned char* a, const float* sf, unsigned char* c, size_t n,
                                                   size_t ngroups, int unroll, const fp8b_shape& sh, int kind)
 {
     constexpr int ES = dt_traits<DST>::size, W = 16 / ES;
     const double rd = __drcp_rn(static_cast<double>(sh.cols));
+    const int jshift = kind == FP8R_ROWS ? 63 : 7;                // one scale per row: j >> 63 = 0
     auto scale_of = [=](size_t e) {
         size_t j;
         const size_t i = fp8b_div(e, sh.cols, rd, j);
-        return sf[kind == FP8B_1X128 ? (j / FP8B_TILE) * sh.rows + i : (i / FP8B_TILE) * sh.l4 + j / FP8B_TILE];
+        return sf[kind != FP8B_128X128 ? (j >> jshift) * sh.rows + i : (i / FP8B_TILE) * sh.l4 + j / FP8B_TILE];
     };
     struct unit { unsigned long long v; float s; };
     cast_tiles(unroll, ngroups * ES, [=](size_t u) { return unit{ld_bits<W>(a + u * W), scale_of(u * W)}; },

@@ -399,27 +399,55 @@ cast_plan plan_fp8_blockwise(uintptr_t a, uintptr_t c, uintptr_t ct, size_t es, 
     return p;
 }
 
-// The argument rules of b200va_quantize_fp8_blockwise after the dtype, format and kind codes, in the order they
-// apply (A of es bytes per element, rows x cols; the caller has checked that the two pairs are each all-NULL or
-// all-non-NULL):
-//   1. with n = rows cols > 0: something requested, dA non-NULL, and n (saturated on overflow) at most 2^40;
-//   2. A aligned to its element size, S and St 4-byte aligned (C and Ct are bytes: any address);
-//   3. no two of A, C, S, Ct and St meeting, the scales' padding included.
-int check_fp8_blockwise_args(size_t es, const void* dA, const void* dC, const float* dS, const void* dCt,
-                             const float* dSt, size_t rows, size_t cols, int kind)
+// The argument rules of b200va_quantize_fp8_blockwise and b200va_quantize_fp8_rowwise after the dtype, format and
+// kind codes, in the order they apply (A of es bytes per element, rows x cols; S and St of sbytes and stbytes; the
+// caller has checked that the two pairs are each all-NULL or all-non-NULL).  The row-wise call's workspace dW of
+// wbytes needs `need` bytes; the blockwise call has none (need = wbytes = 0).
+//   1. with n = rows cols > 0: something requested, dA non-NULL, and n (saturated on overflow) at most 2^40; dW
+//      non-NULL and wbytes >= need;
+//   2. A aligned to its element size, S, St and dW 4-byte aligned (C and Ct are bytes: any address);
+//   3. no two of A, C, S, Ct, St and the needed workspace meeting, the scales' padding included.
+int check_fp8_2d_args(size_t es, const void* dA, const void* dC, const float* dS, size_t sbytes, const void* dCt,
+                      const float* dSt, size_t stbytes, size_t rows, size_t cols, const void* dW = nullptr,
+                      size_t need = 0, size_t wbytes = 0)
 {
     const size_t n = matrix_elems(rows, cols);
-    if (n && ((!dC && !dCt) || !dA || n > (size_t{1} << 40))) return B200VA_ERR_INVALID;
+    if (n && ((!dC && !dCt) || !dA || n > (size_t{1} << 40) || (need && !dW) || wbytes < need)) return B200VA_ERR_INVALID;
     if ((reinterpret_cast<uintptr_t>(dA) & (es - 1)) || (reinterpret_cast<uintptr_t>(dS) & 3u) ||
-        (reinterpret_cast<uintptr_t>(dSt) & 3u))
+        (reinterpret_cast<uintptr_t>(dSt) & 3u) || (reinterpret_cast<uintptr_t>(dW) & 3u))
         return B200VA_ERR_ALIGN;
-    const void* p[5] = {dA, dC, dS, dCt, dSt};
-    const size_t bytes[5] = {n * es, dC ? n : 0, dS ? 4 * b200va_fp8_blockwise_scales(rows, cols, kind) : 0,
-                             dCt ? n : 0, dSt ? 4 * b200va_fp8_blockwise_scales(cols, rows, kind) : 0};
-    for (int x = 0; x < 5; ++x)
-        for (int y = x + 1; y < 5; ++y)
+    const void* p[6] = {dA, dC, dS, dCt, dSt, dW};
+    const size_t bytes[6] = {n * es, dC ? n : 0, dS ? sbytes : 0, dCt ? n : 0, dSt ? stbytes : 0, need};
+    for (int x = 0; x < 6; ++x)
+        for (int y = x + 1; y < 6; ++y)
             if (ranges_meet(p[x], bytes[x], p[y], bytes[y])) return B200VA_ERR_OVERLAP;
     return B200VA_OK;
+}
+
+// The blockwise and row-wise dequantize: one mx_dequant_vec<ES> launch, kind an FP8B_* code or FP8R_ROWS, S of sbytes
+// (the layout's count, 0 when rows cols = 0).  The vector body runs when cols % 16 == 0 and A and C sit on 16-byte
+// boundaries; a unit is a 16-byte output slice, every other element an edge item.
+int dequantize_fp8_2d(int fp8, const void* dA, const float* dS, size_t sbytes, int kind, int dst_dtype, void* dC,
+                      size_t rows, size_t cols, void* stream)
+{
+    if (dst_dtype < 0 || dst_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
+    RC_TRY(current_dev_info(nullptr));
+    const size_t es = dtype_size(dst_dtype), n = matrix_elems(rows, cols);
+    if (n && (!dA || !dS || !dC || n > (size_t{1} << 40))) return B200VA_ERR_INVALID;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC);
+    if ((c & (es - 1)) || (reinterpret_cast<uintptr_t>(dS) & 3u)) return B200VA_ERR_ALIGN;
+    if (ranges_meet(dC, n * es, dA, n) || ranges_meet(dC, n * es, dS, sbytes)) return B200VA_ERR_OVERLAP;
+    if (n == 0) return B200VA_OK;
+    cast_plan p{};
+    if (cols % 16 == 0 && ((a | c) & 15u) == 0) p.ngroups = n / 16;
+    plan_geometry(p, hbm_class(n, es), p.ngroups * es, n - p.ngroups * 16);
+    int rc = B200VA_ERR_VARIANT;
+    with_value<4, 8, 2>(static_cast<int>(es), [&](auto ES) {
+        rc = launch_kernel(mx_dequant_vec<ES>, p.grid, p.threads, 0, static_cast<cudaStream_t>(stream), pdl_enabled(), dA,
+                           static_cast<const void*>(dS), dC, n, p.ngroups, p.unroll, p.prefetch_first, dst_dtype, fp8, 0,
+                           rows, cols, kind);
+    });
+    return rc;
 }
 
 }  // namespace
@@ -564,7 +592,8 @@ int b200va_quantize_fp8_blockwise(int src_dtype, const void* dA, int fp8, int bl
     RC_TRY(current_dev_info(nullptr));
     if (!dC != !dS || !dCt != !dSt) return B200VA_ERR_INVALID;
     const size_t es = dtype_size(src_dtype);
-    RC_TRY(check_fp8_blockwise_args(es, dA, dC, dS, dCt, dSt, rows, cols, block_kind));
+    RC_TRY(check_fp8_2d_args(es, dA, dC, dS, 4 * b200va_fp8_blockwise_scales(rows, cols, block_kind), dCt, dSt,
+                             4 * b200va_fp8_blockwise_scales(cols, rows, block_kind), rows, cols));
     if (rows == 0 || cols == 0) return B200VA_OK;
     size_t smem = 0;
     const cast_plan p = plan_fp8_blockwise(reinterpret_cast<uintptr_t>(dA), reinterpret_cast<uintptr_t>(dC),
@@ -581,26 +610,57 @@ int b200va_quantize_fp8_blockwise(int src_dtype, const void* dA, int fp8, int bl
 int b200va_dequantize_fp8_blockwise(int fp8, const void* dA, const float* dS, int block_kind, int dst_dtype, void* dC,
                                     size_t rows, size_t cols, void* stream)
 {
-    if (dst_dtype < 0 || dst_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT || block_kind < 0 || block_kind >= FP8B_COUNT)
-        return B200VA_ERR_VARIANT;
+    if (block_kind < 0 || block_kind >= FP8B_COUNT) return B200VA_ERR_VARIANT;
+    return dequantize_fp8_2d(fp8, dA, dS, 4 * b200va_fp8_blockwise_scales(rows, cols, block_kind), block_kind, dst_dtype,
+                             dC, rows, cols, stream);
+}
+
+size_t b200va_fp8_rowwise_workspace(size_t rows, size_t cols)
+{
+    return 4 * (b200va_fp8_blockwise_scales(rows, cols, FP8B_1X128) + b200va_fp8_blockwise_scales(cols, rows, FP8B_1X128));
+}
+
+// Three mx_quant_vec<ES> launches chained by PDL, each waiting for the one before: FP8R_MAXIMA (the 1 x 128 block
+// scales into the workspace, under the 1 x 128 blockwise cast's plan), FP8R_REDUCE (one thread per row and column) and
+// FP8R_ROWS (the tiled plan's tiles, or one edge item per element).
+int b200va_quantize_fp8_rowwise(int src_dtype, const void* dA, int fp8, size_t rows, size_t cols, void* dC, float* dS,
+                                void* dCt, float* dSt, void* d_work, size_t work_bytes, void* stream)
+{
+    if (src_dtype < 0 || src_dtype >= DT_COUNT || fp8 < 0 || fp8 >= F8_COUNT) return B200VA_ERR_VARIANT;
     RC_TRY(current_dev_info(nullptr));
-    const size_t es = dtype_size(dst_dtype), n = matrix_elems(rows, cols);
-    if (n && (!dA || !dS || !dC || n > (size_t{1} << 40))) return B200VA_ERR_INVALID;
-    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC);
-    if ((c & (es - 1)) || (reinterpret_cast<uintptr_t>(dS) & 3u)) return B200VA_ERR_ALIGN;
-    const size_t sbytes = 4 * b200va_fp8_blockwise_scales(rows, cols, block_kind);
-    if (ranges_meet(dC, n * es, dA, n) || ranges_meet(dC, n * es, dS, sbytes)) return B200VA_ERR_OVERLAP;
+    if (!dC != !dS || !dCt != !dSt) return B200VA_ERR_INVALID;
+    const size_t es = dtype_size(src_dtype), n = matrix_elems(rows, cols);
+    const size_t need = n <= (size_t{1} << 40) ? b200va_fp8_rowwise_workspace(rows, cols) : 0;
+    RC_TRY(check_fp8_2d_args(es, dA, dC, dS, n ? 4 * rows : 0, dCt, dSt, n ? 4 * cols : 0, rows, cols, d_work, need,
+                             work_bytes));
     if (n == 0) return B200VA_OK;
-    cast_plan p{};
-    if (cols % 16 == 0 && ((a | c) & 15u) == 0) p.ngroups = n / 16;
-    plan_geometry(p, hbm_class(n, es), p.ngroups * es, n - p.ngroups * 16);
+    const uintptr_t a = reinterpret_cast<uintptr_t>(dA), c = reinterpret_cast<uintptr_t>(dC),
+                    ct = reinterpret_cast<uintptr_t>(dCt);
+    size_t smem = 0;
+    const cast_plan pm = plan_fp8_blockwise(a, c, ct, es, rows, cols, FP8B_1X128, smem);
+    cast_plan pr{}, pq = pm;
+    plan_geometry(pr, false, 0, (dC ? rows : 0) + (dCt ? cols : 0));
+    if (!pq.ngroups) plan_geometry(pq, hbm_class(n, es), 0, n);
+    float* w = static_cast<float*>(d_work);
+    float* wt = w + b200va_fp8_blockwise_scales(rows, cols, FP8B_1X128);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     int rc = B200VA_ERR_VARIANT;
     with_value<4, 8, 2>(static_cast<int>(es), [&](auto ES) {
-        rc = launch_kernel(mx_dequant_vec<ES>, p.grid, p.threads, 0, static_cast<cudaStream_t>(stream), pdl_enabled(), dA,
-                           static_cast<const void*>(dS), dC, n, p.ngroups, p.unroll, p.prefetch_first, dst_dtype, fp8, 0,
-                           rows, cols, block_kind);
+        auto launch = [&](const cast_plan& p, size_t sm, const void* A, void* C, void* S, void* Ct, void* St, int kind) {
+            return launch_kernel(mx_quant_vec<ES>, p.grid, p.threads, sm, st, pdl_enabled(), A, C, S, n, p.ngroups, p.unroll,
+                                 0, src_dtype, fp8, 0, 0, Ct, St, rows, cols, kind);
+        };
+        rc = launch(pm, smem, dA, dC, dC ? w : nullptr, dCt, dCt ? wt : nullptr, FP8R_MAXIMA);
+        if (rc == B200VA_OK) rc = launch(pr, 0, w, dS, nullptr, dSt, nullptr, FP8R_REDUCE);
+        if (rc == B200VA_OK) rc = launch(pq, pq.ngroups ? smem : 0, dA, dC, dS, dCt, dSt, FP8R_ROWS);
     });
     return rc;
+}
+
+int b200va_dequantize_fp8_rowwise(int fp8, const void* dA, const float* dS, int dst_dtype, void* dC, size_t rows,
+                                  size_t cols, void* stream)
+{
+    return dequantize_fp8_2d(fp8, dA, dS, rows && cols ? 4 * rows : 0, FP8R_ROWS, dst_dtype, dC, rows, cols, stream);
 }
 
 size_t b200va_dot_workspace_bytes(size_t n)

@@ -532,6 +532,87 @@ def dequantize_fp8_blockwise(q, scales, dtype, *, block: str, out=None, stream=N
     return out
 
 
+def _f32_vector(t, n: int, dev, name: str):
+    """``t`` checked to be a contiguous float32 tensor of n elements on ``dev``, viewed 1-D; or a new one."""
+    torch = _torch()
+    if t is None:
+        return torch.empty(n, dtype=torch.float32, device=dev)
+    if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.numel() != n or t.device != dev
+            or not t.is_contiguous()):
+        raise TypeError(f"{name} must be a contiguous float32 tensor of {n} elements on {dev}")
+    return t.view(n)
+
+
+def quantize_fp8_rowwise(a, fmt, *, rowwise: bool = True, columnwise: bool = True, out=None, scales=None, out_t=None,
+                         scales_t=None, workspace=None, stream=None):
+    """The 2-D ``a`` (rows x cols, contiguous, f32/f64/f16/bf16) quantized to FP8 with one f32 power-of-two scale per
+    row (b200va_quantize_fp8_rowwise), the operands of an H100 row-wise scaled FP8 GEMM.  Per row, k is the largest
+    exponent with amax 2^k <= max finite (amax over the row's finite elements), clamped to [-126, 126]; the scale is
+    2^-k and each element a 2^k rounded once by quantize_fp8's rules.  ``rowwise``: ``out`` ([rows, cols]) and
+    ``scales`` ([rows]); ``columnwise``: ``out_t`` ([cols, rows], A^T's rows) and ``scales_t`` ([cols], one per column
+    of a).  Returns (out, scales, out_t, scales_t), None for a side not asked for.  The scales are 1-D float32, so for a
+    linear layer Y = X W^T, with torch.nn.functional.scaled_mm and ScalingType.RowWise (or torch._scaled_mm):
+
+        Y  = scaled_mm(C_X,  C_W.t(),   scale_a=S_X.view(-1, 1),   scale_b=S_W.view(1, -1))
+        dX = scaled_mm(C_dY, Ct_W.t(),  scale_a=S_dY.view(-1, 1),  scale_b=St_W.view(1, -1))
+        dW = scaled_mm(Ct_dY, Ct_X.t(), scale_a=St_dY.view(-1, 1), scale_b=St_X.view(1, -1))
+
+    where (C_T, S_T, Ct_T, St_T) is this call's result for tensor T, both sides asked for.  ``workspace``: a contiguous
+    CUDA tensor of at least b200va_fp8_rowwise_workspace(rows, cols) bytes, else one is taken from the torch allocator
+    on the call's stream.  Three launches, asynchronous on the current stream."""
+    torch = _torch()
+    src, rows, cols = _matrix(a)
+    dtype, code = _fp8_format(fmt)
+    if not rowwise and not columnwise:
+        raise ValueError("at least one of rowwise and columnwise must be set")
+    if rowwise:
+        out = _out_shaped(out, dtype, (rows, cols), a, "out")
+        scales = _f32_vector(scales, rows, a.device, "scales")
+    else:
+        out = scales = None
+    if columnwise:
+        out_t = _out_shaped(out_t, dtype, (cols, rows), a, "out_t")
+        scales_t = _f32_vector(scales_t, cols, a.device, "scales_t")
+    else:
+        out_t = scales_t = None
+    need = lib.b200va_fp8_rowwise_workspace(rows, cols)
+    if workspace is not None and (not isinstance(workspace, torch.Tensor) or workspace.device != a.device
+                                  or not workspace.is_contiguous()):
+        raise TypeError("workspace must be a contiguous tensor on a's device")
+    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    with torch.cuda.device(a.device):
+        if workspace is None:
+            # allocated on the stream the call runs on, so the allocator reuses it only after that stream's work
+            with torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream()):
+                workspace = torch.empty(max(need, 4), dtype=torch.uint8, device=a.device)
+        check(lib.b200va_quantize_fp8_rowwise(src, a.data_ptr(), code, rows, cols, ptr(out), ptr(scales), ptr(out_t),
+                                              ptr(scales_t), workspace.data_ptr(),
+                                              workspace.numel() * workspace.element_size(), _stream_ptr(stream)),
+              "b200va_quantize_fp8_rowwise")
+    return out, scales, out_t, scales_t
+
+
+def dequantize_fp8_rowwise(q, scales, dtype, *, out=None, stream=None):
+    """The 2-D FP8 ``q`` (rows x cols, torch.float8_e4m3fn / float8_e5m2) with one f32 scale per row (``scales``,
+    rows elements) back to ``dtype`` (b200va_dequantize_fp8_rowwise): q s rounded once, s any f32 (not only a power of
+    two).  For ``out_t`` pass ``scales_t``.  ``out``: a contiguous [rows, cols] tensor of ``dtype`` on q's device, else a
+    new one.  Asynchronous on the current stream."""
+    torch = _torch()
+    code = _operand(q, "q", _fp8_format)
+    if q.dim() != 2:
+        raise TypeError(f"q must be a 2-D tensor, got {q.dim()} dimensions")
+    rows, cols = q.shape
+    dtype, dst = _float_dtype(dtype)
+    if scales is None:
+        raise TypeError("scales must be given")
+    scales = _f32_vector(scales, rows, q.device, "scales")
+    out = _out_shaped(out, dtype, (rows, cols), q, "out")
+    with torch.cuda.device(q.device):
+        check(lib.b200va_dequantize_fp8_rowwise(code, q.data_ptr(), scales.data_ptr(), dst, out.data_ptr(), rows, cols,
+                                                _stream_ptr(stream)), "b200va_dequantize_fp8_rowwise")
+    return out
+
+
 def dot(a, b, *, out=None, workspace=None, stream=None):
     """The reproducible dot product of two equal-length contiguous CUDA tensors of one of f32/f64/f16/bf16
     (b200va_dot): a 0-d float64 CUDA tensor, written asynchronously on the current stream.  The bits

@@ -1,6 +1,6 @@
 """Rate of the cast kernels by family, next to the f32 COPY and READ2 ceiling probes, in one process.
 
-    python tools/cast_rate.py [--family convert|fp8|fp8t|fp8b|mxfp8|sr|all] [--log2n 28] [--calls 20] [--rounds 3]
+    python tools/cast_rate.py [--family convert|fp8|fp8t|fp8b|fp8r|mxfp8|sr|all] [--log2n 28] [--calls 20] [--rounds 3]
                               [--shape ROWSxCOLS]
 
 Per round, every op of the chosen families is timed at n elements with CUDA events around `calls` back-to-back calls
@@ -26,6 +26,12 @@ and the algorithmic bytes of one call:
            A (the yardstick of the row-wise-only case), and the torch-eager recipe for both 1x128 sides (view as
            blocks, amax, exp2 of the scale exponent, multiply, .to(float8); .t().contiguous() and the same again).
            Each entry counts n (sizeof T + outputs) + 4 (scale floats) bytes for what it writes.
+  fp8r     the row-wise quantize at FP8R_SHAPES (or --shape) from each type to E4M3: both sides, row-wise only and
+           column-wise only, and the dequantize of C; beside them at the same shape quantize_fp8_transpose_auto (the
+           same bytes as both sides: A read twice, C and Ct written), quantize_fp8_auto (the same as row-wise only) and
+           the torch-eager recipe for both sides (per-row amax, exp2 of floor(log2(max / amax)), multiply, .to(float8);
+           .t().contiguous() and the same again).  Each entry counts n (sizeof T + outputs) + 4 (scale floats) bytes,
+           A read once, so the rates compare times.
   mxfp8    per type and format, alternated in this order: quantize and dequantize at block 32 and at block 128,
            n * (sizeof T + 1 + 1 / block); the per-tensor recipes they compete with are in the fp8 family.
   sr       the stochastically rounding casts from f32, each beside its round-to-nearest counterpart: to f16 and bf16,
@@ -191,6 +197,53 @@ def fp8b_ops(torch, va, n, tdt, f8, shapes=FP8T_SHAPES):
             del a
 
 
+FP8R_SHAPES = ((16384, 16384), (32768, 4096), (4096, 14336))
+
+
+def fp8r_ops(torch, va, n, tdt, f8, shapes=FP8R_SHAPES):
+    """n is unused: the row-wise family runs at FP8R_SHAPES (or the --shape given)."""
+    f = "e4m3"
+    for rows, cols in shapes:
+        m = rows * cols
+        for s in tdt:
+            a = torch.randn(rows, cols, dtype=torch.float32, device="cuda").to(tdt[s])
+            q = torch.empty(rows, cols, dtype=f8[f], device="cuda")
+            qt = torch.empty(cols, rows, dtype=f8[f], device="cuda")
+            sc = torch.empty(rows, dtype=torch.float32, device="cuda")
+            sct = torch.empty(cols, dtype=torch.float32, device="cuda")
+            ws = torch.empty(va.lib.b200va_fp8_rowwise_workspace(rows, cols), dtype=torch.uint8, device="cuda")
+            back = torch.empty(rows, cols, dtype=tdt[s], device="cuda")
+            amax = torch.zeros(1, dtype=torch.float64, device="cuda")
+            k = torch.zeros(1, dtype=torch.int32, device="cuda")
+            tag = f"{s}->{f} {rows}x{cols}"
+
+            def eager_side(x):
+                amax_r = x.float().abs().nan_to_num(0.0, 0.0, 0.0).amax(dim=1, keepdim=True)
+                kr = torch.floor(torch.log2(448.0 / amax_r)).clamp(-126, 126)
+                return (x.float() * torch.exp2(kr)).to(f8[f]), torch.exp2(-kr).view(-1)
+
+            def eager():
+                eager_side(a)
+                eager_side(a.t().contiguous())
+
+            both = m * (SIZE[s] + 2) + 4 * (rows + cols)
+            yield (f"fp8 rowwise both {tag}",
+                   lambda: va.quantize_fp8_rowwise(a, f, out=q, scales=sc, out_t=qt, scales_t=sct, workspace=ws), both)
+            yield (f"quantize_fp8_transpose_auto {tag}",
+                   lambda: va.quantize_fp8_transpose_auto(a, f, amax=amax, scale_exp=k, out=q, out_t=qt), both)
+            yield (f"fp8 rowwise rowwise {tag}",
+                   lambda: va.quantize_fp8_rowwise(a, f, columnwise=False, out=q, scales=sc, workspace=ws),
+                   m * (SIZE[s] + 1) + 4 * rows)
+            yield (f"quantize_fp8_auto {tag}",
+                   lambda: va.quantize_fp8_auto(a.view(-1), f, amax=amax, scale_exp=k, out=q.view(-1)), m * (SIZE[s] + 1))
+            yield (f"fp8 rowwise columnwise {tag}",
+                   lambda: va.quantize_fp8_rowwise(a, f, rowwise=False, out_t=qt, scales_t=sct, workspace=ws),
+                   m * (SIZE[s] + 1) + 4 * cols)
+            yield f"fp8 rowwise dequantize {tag}", lambda: va.dequantize_fp8_rowwise(q, sc, tdt[s], out=back), m * (SIZE[s] + 1)
+            yield f"torch eager rowwise both {tag}", eager, both
+            del a, q, qt, sc, sct, ws, back, amax, k
+
+
 def mxfp8_ops(torch, va, n, tdt, f8):
     for s in tdt:
         a = torch.randn(n, dtype=torch.float32, device="cuda").to(tdt[s])
@@ -236,7 +289,8 @@ def sr_ops(torch, va, n, tdt, f8):
     del a, amax, c
 
 
-FAMILIES = {"convert": convert_ops, "fp8": fp8_ops, "fp8t": fp8t_ops, "fp8b": fp8b_ops, "mxfp8": mxfp8_ops, "sr": sr_ops}
+FAMILIES = {"convert": convert_ops, "fp8": fp8_ops, "fp8t": fp8t_ops, "fp8b": fp8b_ops, "fp8r": fp8r_ops, "mxfp8": mxfp8_ops,
+            "sr": sr_ops}
 
 
 def main() -> None:
@@ -245,7 +299,7 @@ def main() -> None:
     ap.add_argument("--log2n", type=int, default=28)
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--shape", default=None, help="ROWSxCOLS: run the fp8b family at this shape only")
+    ap.add_argument("--shape", default=None, help="ROWSxCOLS: run the fp8b and fp8r families at this shape only")
     args = ap.parse_args()
 
     import torch
@@ -267,9 +321,9 @@ def main() -> None:
     for r in range(args.rounds):
         for family in families:
             ops = FAMILIES[family]
-            if family == "fp8b" and args.shape:
+            if family in ("fp8b", "fp8r") and args.shape:
                 shape = tuple(int(v) for v in args.shape.split("x"))
-                ops = lambda *x: fp8b_ops(*x, shapes=(shape,))  # noqa: E731
+                ops = lambda *x, f=ops: f(*x, shapes=(shape,))  # noqa: E731
             for op, fn, nbytes in ops(torch, va, n, tdt, f8):
                 report(r, op, timed(fn, args.calls), nbytes)
         x, y, z = (torch.ones(n, dtype=torch.float32, device="cuda") for _ in range(3))
